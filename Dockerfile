@@ -1,4 +1,4 @@
-# CUDA 12.9 devel image + PyTorch; builds the sm_100a extension in-tree at image build time.
+# CUDA 12.9 devel image + PyTorch; builds the sm_90a extension in-tree at image build time.
 FROM nvcr.io/nvidia/pytorch:25.06-py3
 WORKDIR /app
 COPY . /app

@@ -1,4 +1,4 @@
-"""bee2bee_b200 -- Blackwell-native peer-mesh inference engine with the Bee2Bee surface.
+"""bee2bee_b200 -- Hopper (H100) peer-mesh inference engine with the Bee2Bee surface.
 
 Public exports mirror the reference package (/root/reference/bee2bee/__init__.py:1-11):
 ``P2PNode``, ``run_p2p_node``, ``api_server`` (the FastAPI module) and ``__version__``.

@@ -1,7 +1,7 @@
 """``bee2bee`` command line (parity: /root/reference/bee2bee/__main__.py:30-123).
 
 Same verbs and options (``serve-ollama``, ``serve-hf``, ``serve-hf-remote``, ``register``)
-plus what a B200 deployment needs: ``--pieces`` (layer pieces = GPUs), ``config``,
+plus what a H100 deployment needs: ``--pieces`` (layer pieces = GPUs), ``config``,
 ``topology``, ``bench``.  ``register``'s handshake test really connects and measures a ping
 round-trip (the reference sleeps 1.5 s and prints success).
 """
@@ -40,7 +40,7 @@ def _configure_logging() -> None:
 
 @click.group()
 def cli():
-    """Bee2Bee on B200: peer-mesh inference over NVLink."""
+    """Bee2Bee on H100: peer-mesh inference over NVLink."""
     _configure_logging()
 
 

@@ -1,10 +1,10 @@
-"""In-tree build of the native extension ``bee2bee_b200/_C*.so`` for sm_100a.
+"""In-tree build of the native extension ``bee2bee_b200/_C*.so`` for sm_90a (H100).
 
 Plain ``nvcc`` for the kernel translation units (no torch headers -> seconds each),
 ``g++`` for the single torch-facing binding, one link step.  Objects are cached by a
 content hash under ``build/`` so repeated ``build()`` calls are incremental.  The
-resulting ``.so`` lives inside the package so that it travels with the tree to the GPU
-box (no JIT cache under ``~/.cache``).
+resulting ``.so`` lives inside the package, so the tree is importable as built (no JIT cache
+under ``~/.cache``).
 """
 from __future__ import annotations
 
@@ -26,7 +26,7 @@ CU_SOURCES = ["gemm_tc.cu", "elementwise.cu", "attention.cu", "attention_tc.cu",
 CPP_SOURCES = ["peer.cpp", "binding.cpp"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 
@@ -88,7 +88,7 @@ def build(verbose: bool = True, force: bool = False) -> Path:
 
     if jobs:
         if verbose:
-            print(f"[bee2bee_b200] compiling {len(jobs)} translation unit(s) for sm_100a ...", flush=True)
+            print(f"[bee2bee_b200] compiling {len(jobs)} translation unit(s) for sm_90a ...", flush=True)
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(lambda j: _run(*j), jobs))
 

@@ -14,7 +14,7 @@ DEFAULT_CONFIG: Dict[str, Any] = {
     "bootstrap_url": "ws://127.0.0.1:4003",
     "p2p_port": 0,
     "api_port": 4002,
-    # engine (B200) defaults
+    # engine (H100) defaults
     "pieces": 1,
     "max_batch": 32,
     "max_seq_len": 4096,

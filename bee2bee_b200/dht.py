@@ -2,7 +2,7 @@
 
 Same async surface (``DHTNode.start/set/get``, ``announce_piece``, ``find_providers``).
 Backends: Kademlia over UDP when the optional ``kademlia`` package exists and the node is
-not offline; otherwise an in-process table.  On the B200 box every peer lives on one host,
+not offline; otherwise an in-process table.  On the H100 box every peer lives on one host,
 so ``MeshDHT`` resolves keys from the NVLink topology (layer piece -> rank/device) without
 any network -- this is what ``P2PNode`` wires in (the reference never wires its DHT)."""
 from __future__ import annotations

@@ -78,7 +78,7 @@ def deserialize_layer(d: Dict) -> Layer:
 
 # ------------------------------------------------------------------ device path
 def _tc_ok(dev, *dims_128, k: int) -> bool:
-    """the tcgen05 swap-AB GEMM applies: CUDA device, output features multiple of 128, reduction multiple of 64"""
+    """the wgmma swap-AB GEMM applies: CUDA device, output features multiple of 128, reduction multiple of 64"""
     import torch
 
     if not str(dev).startswith("cuda") or not torch.cuda.is_available():
@@ -88,7 +88,7 @@ def _tc_ok(dev, *dims_128, k: int) -> bool:
 
 
 def _tc_matmul(a, b_t, bias=None):
-    """a [T, K] @ b_t[N, K]^T -> fp32 [T, N] on the tcgen05 GEMM (bf16 operands, fp32 accumulate, fp32 out)"""
+    """a [T, K] @ b_t[N, K]^T -> fp32 [T, N] on the wgmma GEMM (bf16 operands, fp32 accumulate, fp32 out)"""
     import torch
     from . import ops
 
@@ -97,8 +97,8 @@ def _tc_matmul(a, b_t, bias=None):
 
 
 def dense_forward_device(W, b, activation: str, x, device=None):
-    """torch tensors in, (y, z) out; runs on ``device`` (GPU when available).  On a B200 with tile-aligned shapes
-    the product runs on the tcgen05 GEMM (bf16 operands, fp32 accumulation, bias fused in the epilogue) -- K12."""
+    """torch tensors in, (y, z) out; runs on ``device`` (GPU when available).  On a H100 with tile-aligned shapes
+    the product runs on the wgmma GEMM (bf16 operands, fp32 accumulation, bias fused in the epilogue) -- K12."""
     import torch
 
     dev = device or ("cuda" if torch.cuda.is_available() else "cpu")

@@ -281,11 +281,12 @@ def piece_units(cfg: "ModelConfig", pieces: int, bounds: Optional[List[int]] = N
     pieces = max(1, min(pieces, cfg.n_layers))
     if pieces == 1 or not supports_half_layer_pieces(cfg):
         return [(UPL * r.start, UPL * r.stop) for r in balanced_split(cfg, pieces)]
-    # stage time model fitted to the measured decode step (profiles/decode_layer_breakdown.md, B200, 32 sequences):
-    # weight bytes at the measured 6.4 TB/s plus a fixed cost per kernel; the last piece adds the lm_head GEMM and the
-    # sampler.  Llama-3-8B: attention block 34.1 us (measured 34.7), gate/up 40.7 (39.4), down 25.3 (24.9), head 201 (211).
+    # stage time model of a decode step: weight bytes at an effective 6.4 TB/s plus a fixed cost per kernel; the last
+    # piece adds the lm_head GEMM and the sampler.  These constants are not measured on H100 (data-sheet HBM3: 3.35
+    # TB/s).  The boundaries depend on them: the streaming rate sets how much a weight byte costs against the fixed
+    # per-kernel cost, so a different rate can move a cut.
     h, f = cfg.hidden_size, cfg.ffn_size
-    us_per_elem = 2.0 / 6.4e6                            # bf16 element -> microseconds of HBM streaming
+    us_per_elem = 2.0 / 6.4e6                            # bf16 element -> microseconds of weight streaming
     launch = 7.0
     attn = (h * (cfg.q_dim + 2 * cfg.kv_dim) + cfg.q_dim * h) * us_per_elem + 3 * launch
     gu = 2 * h * f * us_per_elem + 4.0

@@ -1,5 +1,5 @@
-"""One *piece* (contiguous layer range) resident on one B200, executed entirely by the
-hand-written sm_100a kernels in ``csrc/``.
+"""One *piece* (contiguous layer range) resident on one H100, executed entirely by the
+hand-written sm_90a kernels in ``csrc/``.
 
 Per decoder layer (Llama / Mistral) exactly five launches, all on one stream:
 
@@ -112,7 +112,7 @@ class NativePiece:
         self.fused_norm = cfg.norm == "rms"
         # W8A8 e4m3 (Llama / Mistral graphs).  "fp8": per-output-row weight scales x per-token activation scales
         # applied in the epilogue; "mxfp8": OCP-MX block scaling, one UE8M0 scale per 32 K elements on both
-        # operands, applied by the tensor core (tcgen05 kind::mxf8f6f4.block_scale).
+        # operands, applied by the GEMM to each 32-K partial product.
         self.fp8 = quant in ("fp8", "mxfp8") and self.fused_norm and not cfg.post_norms and cfg.glu
         self.mx = self.fp8 and quant == "mxfp8"
         self.mx_fuse = False

@@ -1,7 +1,7 @@
 """Plain-PyTorch implementation of every supported decoder family.
 
 Two jobs: (1) the numerical oracle every CUDA kernel / fused path is tested against, and
-(2) the execution backend on machines without a B200 (CPU plumbing config of
+(2) the execution backend on machines without a H100 (CPU plumbing config of
 BASELINE.json: distilgpt2 split in two pieces over the loopback mesh).  Semantics follow
 the Hugging Face modelling code the reference delegates to
 (/root/reference/bee2bee/hf.py:23-44).

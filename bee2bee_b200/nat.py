@@ -2,7 +2,7 @@
 STUN, public-IP discovery with a 5-minute cache, status/manual-instruction helpers and the
 legacy wrappers (``try_upnp_map``, ``try_stun``, ``auto_port_forward``, ``get_public_ip``).
 
-On the B200 box peers are GPUs of one host: reachability is a CUDA peer-access question
+On the H100 box peers are GPUs of one host: reachability is a CUDA peer-access question
 answered by ``parallel.mesh``; this module exists so WAN deployments keep working and is
 completely inert when ``BEE2BEE_OFFLINE`` is set (no sockets are opened)."""
 from __future__ import annotations

@@ -12,7 +12,7 @@ longer exists, so nothing can drive it.  Here:
   ``run_train_step`` / ``run_hf_pipeline`` built on TASK/RESULT frames, so the protocol
   constants that have no implementation anywhere in the reference are actually usable.
 
-On a B200 mesh the product path does not use any of this (pieces hand off over NVLink);
+On a H100 mesh the product path does not use any of this (pieces hand off over NVLink);
 it is kept for surface parity and as a CPU-cluster fallback.
 """
 from __future__ import annotations
@@ -161,7 +161,7 @@ class TaskExecutor:
         model_id = p.get("model_id") or new_id("hfpart")
         device = str(p.get("device") or self.device)
         if device.startswith("cuda") and cfg.norm == "rms" and cfg.glu:
-            # B200 data plane: the layer range runs on the hand-written kernels with a paged KV cache, and hop payloads
+            # H100 data plane: the layer range runs on the hand-written kernels with a paged KV cache, and hop payloads
             # may stay in device memory (hidden_ref: cudaMemcpyPeerAsync / CUDA IPC instead of JSON lists)
             import torch
             from .engine.tokenizer import load_tokenizer

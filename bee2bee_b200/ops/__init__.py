@@ -1,4 +1,4 @@
-"""Python face of the hand-written sm_100a kernels (``csrc/*.cu`` -> ``bee2bee_b200/_C``).
+"""Python face of the hand-written sm_90a kernels (``csrc/*.cu`` -> ``bee2bee_b200/_C``).
 
 Every function here launches a native kernel on the current CUDA stream.  There is no
 silent PyTorch fallback on a GPU box: if the extension is missing, ``native()`` raises.
@@ -16,7 +16,7 @@ import torch
 
 EPI_PLAIN, EPI_RESIDUAL, EPI_GLU, EPI_QKV_ROPE, EPI_GELU = 0, 1, 2, 3, 4
 PAGE = 64           # tokens per KV page (csrc/attention.cu)
-NUM_SMS = 148
+NUM_SMS = 132      # H100 SXM
 
 _C = None
 
@@ -79,7 +79,7 @@ def _ptr(t: Optional[torch.Tensor]) -> int:
 # ------------------------------------------------------------------ weight prep
 def rope_interleave_rows(w: torch.Tensor, n_heads: int, head_dim: int) -> torch.Tensor:
     """Row permutation inside each head: new row 2j <- old j, 2j+1 <- old j + D/2, so a rotary
-    pair sits in adjacent TMEM lanes of the QKV GEMM epilogue.  q.k dot products are invariant
+    pair sits in adjacent lanes (output rows) of the QKV GEMM epilogue.  q.k dot products are invariant
     under the (shared) permutation, so attention is unchanged."""
     half = head_dim // 2
     idx = torch.arange(head_dim, device=w.device).view(2, half).t().reshape(-1)   # [0, half, 1, half+1, ...]
@@ -124,17 +124,14 @@ PREFILL_SPLITK = os.environ.get("B2B_PREFILL_SPLITK", "1") == "1"
 
 
 def pick_prefill_tile(n_out: int, m_tok: int, k: int = 0):
-    """(token tile, ring depth, cluster split-K) of a prefill GEMM (m_tok > 64), measured on B200 on the Llama-3-8B shapes
-    (profiles/prefill_gemm.md).  0 = the tile's default depth / let ``pick_splitk`` decide.
+    """(token tile, ring depth, cluster split-K) of a prefill GEMM (m_tok > 64) on the Llama-3-8B shapes.  0 = the
+    tile's default depth / let ``pick_splitk`` decide.
 
-    * more tiles than SMs: TWO resident CTAs per SM with a shallow ring beat one CTA with a deep ring -- the epilogue of
-      one tile (TMEM -> registers -> global) overlaps the main loop of the other (955 vs 787 TFLOP/s over the layer at
-      4096 tokens, 570 vs 551 at 512);
+    * more tiles than SMs: a shallow ring, so that a ring's worth of shared memory per tile stays small;
     * fewer tiles than SMs (O-proj / down / QKV of a 256-1024 token chunk: 32-48 weight tiles): fill the machine with
-      split-K instead of running 2 waves of deep-ring CTAs.  Long K (down, 14336): 256-wide token tiles (the 128x256 MMA
-      runs at full rate, 128x128 does not), one CTA per SM, split-K until ~one CTA per SM (512 tokens: 66.9 vs 109.5 us).
-      Short K: 128-wide tiles with a 3-deep ring, two CTAs per SM, split-K until ~two CTAs per SM (O-proj, 512 tokens:
-      37.1 vs 55.7 us).  At least 32 k-blocks per CTA, split-K <= 4."""
+      split-K instead of running 2 waves of deep-ring CTAs.  Long K (down, 14336): 256-wide token tiles, split-K until
+      ~one CTA per SM.  Short K: 128-wide tiles with a 3-deep ring, split-K until ~two CTAs per SM.  At least 32
+      k-blocks per CTA, split-K <= 4."""
     tn = n_out // 128
     tiles256 = tn * ((m_tok + 255) // 256)
     tiles128 = tn * ((m_tok + 127) // 128)
@@ -157,13 +154,11 @@ def pick_prefill_tile(n_out: int, m_tok: int, k: int = 0):
     return (128 if m_tok <= 512 else 256), 0, 0          # small chunks: not measured, the decode heuristic decides
 
 
-#: cluster size of the TMA-multicast prefill GEMM (2 or 4); correct on hardware but NOT faster (the prefill GEMM is not
-#: L2-bound, profiles/prefill_gemm.md), so default off;
+#: cluster size of the TMA-multicast prefill GEMM (2 or 4), default off;
 #: applies to bf16 GEMMs with token tiles of 128 / 256 and no split-K, everything else ignores it
 GEMM_MC = int(os.environ.get("B2B_GEMM_MC", "0"))
 
-#: L2 weight prefetch: built, measured negative and REMOVED from the kernel in round 2 (profiles/l2_prefetch.md; even
-#: switched off its code and parameters cost ~20 us per decode step).  The value is accepted and ignored.
+#: L2 weight prefetch: not part of the kernel; the value is accepted and ignored.
 L2_PREFETCH = 0
 
 #: shared-memory ring depth of the decode GEMMs (0 = per-token-tile default); fewer stages -> more CTAs per SM, so the
@@ -183,9 +178,8 @@ def pick_splitk(n_out: int, m_tok: int, k: int, bn: int, epi: int, stages: int =
     if (n_out, k) in SPLITK_OVERRIDE:
         want = SPLITK_OVERRIDE[(n_out, k)]
     else:
-        # measured (tools/layer_sweep.py, Llama-3-8B, reduce-scatter split-K epilogue): up to ~2 CTAs per SM pay off
-        # (bn=32: qkv 4, o 4, gate/up 1, down 8 -> 100 us/layer; bn=16: 4/4/1/4 -> 92.6 us); >= 16 k-blocks per
-        # CTA, and every CTA of the cluster keeps >= 4 token columns (vector DSMEM stores)
+        # up to ~2 CTAs per SM (Llama-3-8B decode, bn=32: qkv 4, o 4, gate/up 1, down 8; bn=16: 4/4/1/4); >= 16
+        # k-blocks per CTA, and every CTA of the cluster keeps >= 4 token columns
         tiles = (n_out // 128) * ((m_tok + bn - 1) // bn)
         limit = 256 if bn >= 32 else 200
         want = 1
@@ -215,7 +209,7 @@ def gemm(w: torch.Tensor, x: torch.Tensor, out: Optional[torch.Tensor] = None, *
          fq_out: Optional[torch.Tensor] = None, fq_sf: Optional[torch.Tensor] = None, fq_bn: int = 0,
          sumsq_out: Optional[torch.Tensor] = None, zero_buf: Optional[torch.Tensor] = None,
          sumsq: Optional[torch.Tensor] = None, no_out: bool = False) -> Optional[torch.Tensor]:
-    """out[t, n] = epilogue(sum_k x[t, k] * w[n, k]) on the tcgen05 swap-AB kernel."""
+    """out[t, n] = epilogue(sum_k x[t, k] * w[n, k]) on the wgmma swap-AB kernel."""
     m_tok, k = x.shape
     n_out = w.shape[0]
     if bn <= 0:
@@ -285,7 +279,7 @@ def quant_fp8_rows(x: torch.Tensor, eps: float = 1e-5, with_rms: bool = False, o
 
 
 # ------------------------------------------------------- MX (block-scaled) fp8
-MX_BLOCK = 32          # K elements per UE8M0 scale (OCP MX / tcgen05 kind::mxf8f6f4.block_scale)
+MX_BLOCK = 32          # K elements per UE8M0 scale (OCP MX)
 
 
 def pick_bn_mx(m_tok: int) -> int:
@@ -294,7 +288,7 @@ def pick_bn_mx(m_tok: int) -> int:
 
 
 def mx_chunk_layout(sf: torch.Tensor, rows_per_tile: int = 128) -> torch.Tensor:
-    """[R, K/32] scale bytes (R multiple of 128, K multiple of 128) -> the tcgen05.cp chunk layout
+    """[R, K/32] scale bytes (R multiple of 128, K multiple of 128) -> the GEMM's scale-factor chunk layout
     [R/128][K/128][32 (r % 32)][4 (r / 32)][4 (k-block in chunk)] flattened (512 bytes per chunk)."""
     R, nb = sf.shape
     assert R % 128 == 0 and nb % 4 == 0
@@ -391,11 +385,9 @@ def add(a, b, out=None):
 # -------------------------------------------------------------------- attention
 def attention(q, k_cache, v_cache, out, block_table, q_start, q_len, kv_len, *, max_q, n_q, n_kv, head_dim,
               window=0, softcap=0.0, splits=1, ws=None, use_tc=-1, fq_out=None, fq_sf=None, fq_bn=0):
-    """Paged-KV attention.  Prefill chunks (max_q >= 2) run on the tcgen05 flash kernel.  Decode (max_q == 1) also does
-    when the batch fills the machine (sequences x kv heads >= 128 CTAs) or no split-KV was asked for: measured on B200
-    (profiles/decode_attention.md) it streams the KV pages at 0.66 of the HBM peak at 8k context against 0.49 for the
-    CUDA-core split-KV kernel, and is faster even at 64 tokens (7.9 vs 10.1 us); few sequences with a long context
-    keep the split-KV kernel (more CTAs than (sequence, kv head) pairs)."""
+    """Paged-KV attention.  Prefill chunks (max_q >= 2) run on the tensor-core flash kernel, and so does decode
+    (max_q == 1) unless ``use_tc`` = 0 selects the CUDA-core kernel; with ``splits`` > 1 every (sequence, kv head,
+    split) CTA streams its share of the pages and a merge pass combines the partials."""
     if use_tc < 0 and max_q == 1:
         # split-KV (few sequences x long context) also runs on the tensor-core kernel: every (sequence, kv head, split) CTA
         # streams its share of the pages, the shared merge pass combines the partials
@@ -408,7 +400,7 @@ def attention(q, k_cache, v_cache, out, block_table, q_start, q_len, kv_len, *, 
 
 
 def attention_fuses_quant(max_q: int, n_q: int, n_kv: int, head_dim: int, splits: int) -> bool:
-    """True when ``attention`` will run the tcgen05 kernel without split-KV, i.e. can emit the e4m3 copy itself."""
+    """True when ``attention`` will run the tensor-core kernel without split-KV, i.e. can emit the e4m3 copy itself."""
     g = n_q // max(1, n_kv)
     tc_ok = n_kv > 0 and n_q % n_kv == 0 and g in (1, 2, 4, 8, 16) and head_dim in (64, 128, 256) and get_attn_tc_min_q() > 0
     if not tc_ok:
@@ -417,7 +409,7 @@ def attention_fuses_quant(max_q: int, n_q: int, n_kv: int, head_dim: int, splits
 
 
 def set_attn_tc_min_q(n: int) -> None:
-    """Query-chunk length from which prefill attention runs on the tcgen05 kernel (0 = scalar kernel only)."""
+    """Query-chunk length from which prefill attention runs on the tensor-core kernel (0 = scalar kernel only)."""
     native().set_attn_tc_min_q(int(n))
 
 

@@ -10,7 +10,7 @@ to decoder LMs with a KV cache:
 * ``MeshPipelineService``  an ``hf``-shaped service on the head peer that drives generation
                            through the chain piece0 (local) -> piece1 (remote) -> ... and samples.
 
-On a B200 box this path is not used: pieces hand activations GPU->GPU (``parallel.mesh``).
+On a H100 box this path is not used: pieces hand activations GPU->GPU (``parallel.mesh``).
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Layer range [start, end) of a decoder LM resident on ONE B200 for the legacy coordinator / worker protocol
+"""Layer range [start, end) of a decoder LM resident on ONE H100 for the legacy coordinator / worker protocol
 (``hf_part_load`` / ``hf_part_forward``, /root/reference/bee2bee/node.py:236-277), executed by the hand-written
 kernels (``NativePiece``) with a paged KV cache per session.
 

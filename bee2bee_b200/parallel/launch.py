@@ -1,4 +1,4 @@
-"""Multi-GPU serving launcher: ``serve-hf --pieces N`` on a B200 box.
+"""Multi-GPU serving launcher: ``serve-hf --pieces N`` on a H100 box.
 
 Rank 0 is the process the user started (mesh node + HTTP sidecar + scheduler); ranks 1..N-1
 are spawned as ``python -m bee2bee_b200.parallel.launch --follower`` subprocesses, one per GPU.

@@ -1,6 +1,6 @@
 """NVLink mesh: the in-process replacement for the reference's WAN discovery and transport.
 
-``peer = one B200 hosting one piece``.  What the reference does with bootstrap links,
+``peer = one H100 hosting one piece``.  What the reference does with bootstrap links,
 hello/peer_list gossip, DHT lookups, STUN/UPnP and one WebSocket per peer pair
 (/root/reference/bee2bee/p2p_runtime.py:308-372,478-523; dht.py; nat.py) collapses into
 

@@ -6,7 +6,7 @@
 Result / metadata keys and stream formats are the reference's (NDJSON ``{"text":..}``
 lines + ``{"done": true}`` for HF, raw text chunks for Ollama).  What differs is what is
 behind them: ``HFService`` enqueues into this framework's continuous-batching engine
-(hand-written sm_100a kernels, pieces across GPUs) instead of calling
+(hand-written sm_90a kernels, pieces across GPUs) instead of calling
 ``transformers.generate`` inline, and every service exposes ``aexecute`` /
 ``aexecute_stream`` so asyncio callers never block their loop (SURVEY section 8).
 """
@@ -165,7 +165,7 @@ class HFService(BaseService):
 # ========================================================================================== Ollama
 class EmbeddedOllama:
     """In-process stand-in for an Ollama daemon with the same JSON shapes (``/api/tags``,
-    ``/api/generate``).  There is no ``ollama`` binary on the B200 box (and no network to pull
+    ``/api/generate``).  There is no ``ollama`` binary on the H100 box (and no network to pull
     models), so ``serve-ollama`` serves the requested model through the native engine while
     keeping the Ollama request/response contract."""
 

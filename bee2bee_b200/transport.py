@@ -2,7 +2,7 @@
 
 * ``ws://`` / ``wss://``  -- ``websockets`` text frames, 32 MiB cap: wire-compatible with the
   reference mesh and its JS bridge (/root/reference/bee2bee/p2p_runtime.py:174-179,350).
-* ``inproc://``           -- an in-process hub (pairs of asyncio queues).  On one B200 box all
+* ``inproc://``           -- an in-process hub (pairs of asyncio queues).  On one H100 box all
   peers live in one host, so the control plane does not need sockets at all; also what the
   multi-peer unit tests use (no ports, no NAT probing).
 

@@ -1,4 +1,4 @@
-"""Address discovery (parity: /root/reference/bee2bee/utils.py:68-98).  On the B200 box the
+"""Address discovery (parity: the reference's bee2bee/utils.py:68-98).  On the H100 box the
 mesh is node-local, so WAN probing is skipped whenever ``BEE2BEE_OFFLINE`` is set."""
 from __future__ import annotations
 

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Headline benchmark (BASELINE.json): decode tokens/s + p50 TTFT for Llama-3-8B (bf16,
-random-init weights, synthetic 16-token prompts) split into N pieces on N B200s.
+random-init weights, synthetic 16-token prompts) split into N pieces on N H100s.
 
     python bench.py --gpus 1 --steps 64 --warmup 8
+    python bench.py --gpus 1 --steps 64 --warmup 8 --dump-outputs DIR   # + last step's tokens / logits as .npy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...     # A: the unmodified reference (baseline/_ref), HFService path
@@ -56,7 +57,11 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--dtype", default=None, choices=["bf16", "fp8", "mxfp8"],
                     help="fp8 = W8A8 e4m3 GEMMs with per-row/per-token scales; mxfp8 = block-scaled (UE8M0 per 32 K) "
-                         "tcgen05 kind::mxf8f6f4 GEMMs (secondary configs)")
+                         "e4m3 GEMMs (secondary configs)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (sampled token of every "
+                         "sequence, fp32 logits of the group that ran last) to DIR/<name>.npy, 64 MB at most; the "
+                         "inputs are seeded, so runs with the same arguments can be compared output for output")
     a = ap.parse_args()
     cfg = CONFIGS[a.config]
     dflt = dict(model="llama-3-8b", dtype="bf16", batch=32, groups=0, prompt_len=16, steps=64, warmup=8)
@@ -153,9 +158,39 @@ def gather_objects(obj, world):
 def common_fields(args, world, total, K, W, P, extra_cfg):
     cfgd = {"model": args.model, "global_batch": total, "seq_len": P + W + K, "prompt_len": P, "pieces": world,
             "baseline_config": args.config, "weights": "random-init", "sampling": "T=0.7 top_p=0.95 rep=1.15",
-            "l2": "per-step weight stream (>= 1.7 GB/GPU) exceeds the 126 MB L2; a 256 MB buffer is written before timing"}
+            "l2": "per-step weight stream (>= 1.7 GB/GPU) exceeds the 50 MB L2; a 256 MB buffer is written before timing"}
     cfgd.update(extra_cfg)
     return cfgd
+
+
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, runner, win, total, vocab, rank):
+    """What the last timed decode step handed back, as float32 / float64 .npy files of at most 64 MB in all:
+    tokens.npy      [total] the token every sequence sampled in the last step;
+    logits.npy      [rows, vocab] fp32 logits of that step.  The last piece keeps one logits buffer that every
+                    micro-batch group overwrites in turn, so the rows are those of the group that ran last (every
+                    sequence when there is one group, the default on one GPU), cut to a fixed, seeded row sample when
+                    they would exceed the size cap;
+    logits_rows.npy [rows] the sequence index of each logits row."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    tokens_bytes = total * 8
+    if runner.last:
+        g = runner.groups - 1
+        seqs = np.arange(g * runner.gb, (g + 1) * runner.gb)
+        rows = np.arange(runner.gb)
+        max_rows = max(1, (DUMP_CAP_BYTES - tokens_bytes - 8 * len(rows) - 1024) // (vocab * 4 + 8))
+        if len(rows) > max_rows:
+            rows = np.sort(np.random.default_rng(0).choice(len(rows), size=max_rows, replace=False))
+        logits = runner.piece.logits[torch.as_tensor(rows, dtype=torch.long), :vocab].float().cpu().numpy()
+        np.save(os.path.join(out_dir, "logits.npy"), logits)
+        np.save(os.path.join(out_dir, "logits_rows.npy"), seqs[rows].astype(np.float64))
+    if rank == 0:
+        np.save(os.path.join(out_dir, "tokens.npy"), win[:, -1].cpu().numpy().astype(np.float64))
 
 
 # ----------------------------------------------------------------------------- ours (C)
@@ -214,7 +249,7 @@ def run_ours(args):
     runner.sync()
     barrier_sync()
     launches0 = runner.kernel_launches
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
     flush.fill_(1)
     barrier_sync()
     sampler.mark()                         # clocks are reported from the samples taken during the timed region
@@ -227,6 +262,8 @@ def run_ours(args):
     clocks = sampler.stop() if rank == 0 else {}
     launches = runner.kernel_launches - launches0
     win = runner.fetch_window([0] * total, 1 + W + K)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, runner, win, total, cfg.vocab_size, rank)
     uniq = 0
     if rank == 0:
         assert int((win >= 0).all()) and int((win < cfg.vocab_size).all()), "sampler produced out-of-range ids"

@@ -1,4 +1,4 @@
-// Paged-KV attention for sm_100a (decode + chunked prefill), GQA-aware.
+// Paged-KV attention for sm_90a (decode + chunked prefill), GQA-aware.
 //
 // One CTA = (sequence, kv head, query block [, kv split]).  All G = n_q/n_kv query
 // heads that share the kv head are processed together, so each K/V page is read from

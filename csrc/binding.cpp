@@ -276,7 +276,7 @@ void attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, co
   c10::cuda::CUDAGuard guard(q.device());
   TORCH_CHECK(block_table.scalar_type() == at::kInt && q_len.scalar_type() == at::kInt, "int32 metadata expected");
   const int seqs = static_cast<int>(q_len.size(0));
-  // use_tc: -1 = by query-chunk length (prefill chunks), 1 = force the tcgen05 kernel (decode: one-token query blocks,
+  // use_tc: -1 = by query-chunk length (prefill chunks), 1 = force the tensor-core kernel (decode: one-token query blocks,
   // the GQA group stacked into the MMA rows), 0 = force the CUDA-core kernel (split-KV decode of few sequences)
   const bool want_tc = use_tc < 0 ? (max_q >= g_attn_tc_min_q && g_attn_tc_min_q > 0) : (use_tc > 0 && g_attn_tc_min_q > 0);
   if (want_tc && splits > 1 && max_q == 1) {
@@ -286,7 +286,7 @@ void attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, co
   }
   if (want_tc &&
       b2b::attention_tc_supported(static_cast<int>(n_q), static_cast<int>(n_kv), static_cast<int>(head_dim))) {
-    // prefill chunk: tcgen05 flash attention
+    // prefill chunk: tensor-core flash attention
     check(b2b::launch_attention_tc(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(),
                                    reinterpret_cast<const int*>(block_table.data_ptr()),
                                    reinterpret_cast<const int*>(q_start.data_ptr()),
@@ -300,7 +300,7 @@ void attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, co
           "attention_tc");
     return;
   }
-  TORCH_CHECK(fq_out == 0, "fused output quantisation needs the tcgen05 attention kernel");
+  TORCH_CHECK(fq_out == 0, "fused output quantisation needs the tensor-core attention kernel");
   if (splits > 1) {
     TORCH_CHECK(ws.has_value(), "split-KV needs a workspace");
     const int64_t R = b2b::attn_rows(static_cast<int>(n_q / n_kv), 1);
@@ -416,7 +416,7 @@ Tensor tensor_from_ptr(int64_t p, std::vector<int64_t> sizes, const std::string&
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "bee2bee_b200 native sm_100a kernels + NVLink peer-memory runtime";
+  m.doc() = "bee2bee_b200 native sm_90a kernels + NVLink peer-memory runtime";
   m.def("gemm", &gemm);
   m.def("gemm_max_splitk", &gemm_max_splitk);
   m.def("init_kernels", &init_kernels);

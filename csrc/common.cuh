@@ -1,6 +1,6 @@
-// Shared sm_100a device helpers: mbarrier, TMA, tcgen05/TMEM, cluster/DSMEM,
+// Shared sm_90a device helpers: mbarrier, TMA, wgmma operand descriptors, cluster/DSMEM,
 // system-scope flags for the NVLink piece handoff.  Everything is inline PTX —
-// no CUTLASS dependency.  Bit layouts follow the PTX ISA tcgen05 descriptors.
+// no CUTLASS dependency.  Bit layouts follow the PTX ISA wgmma descriptors.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -120,134 +120,33 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   return p;
 }
 
-// ------------------------------------------------------------ tcgen05 / TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM cols: pow2 in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate; single CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// fp8 (e4m3) inputs, fp32 accumulate (kind::f8f6f4, non block-scaled).
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// MX block-scaled fp8: e4m3 x e4m3 with one UE8M0 scale per 32 K elements; the scale factors live in
-// TMEM (4 columns per 128 rows x 4 k-blocks; the descriptor's sf-id fields pick the k-block byte).
-__device__ __forceinline__ void umma_mxf8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate, uint32_t sfa_tmem, uint32_t sfb_tmem) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}\n"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(sfa_tmem), "r"(sfb_tmem)
-      : "memory");
-}
-// smem -> TMEM copy of 32 rows x 16 bytes, replicated into the four 32-lane subpartitions (scale factors).
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-// un-swizzled K-major descriptor of a contiguous [32 rows][16 bytes] scale-factor chunk (8-row atoms 128 B apart)
-__device__ __forceinline__ uint64_t make_sf_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(128 >> 4) << 32;               // SBO: next 8-row atom
-  d |= static_cast<uint64_t>(1) << 46;
-  return d;
-}
 // 1D bulk copy global -> shared with mbarrier transaction accounting (size multiple of 16 bytes)
 __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// tcgen05.commit: arrive on an mbarrier once all previously issued MMAs retire.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// Same, arriving on the mbarrier at this offset in every CTA of `cta_mask` (a stage that is filled by multicast
-// may only be refilled once ALL consumers of the cluster have retired their MMAs on it).
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-// Each thread of the warp reads its own TMEM lane (warp%4 selects the 32-lane
-// quarter via the address), 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 
-// K-major, 128B-swizzled shared-memory operand descriptor (rows of 128 bytes,
-// 8-row x 128B swizzle atoms stacked every 1024 bytes).
+// ------------------------------------------------------------ wgmma shared-memory operand descriptors
+// K-major, 128B-swizzled operand (rows of 128 bytes, 8-row x 128B swizzle atoms stacked every 1024 bytes).  Inside
+// the atom, advancing 32 bytes along K is +2 on the descriptor (the start address field counts 16-byte units).
 __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);   // start address   [0,14)
-  d |= static_cast<uint64_t>(1) << 16;                       // LBO (ignored for swizzled K-major)
+  d |= static_cast<uint64_t>(1) << 16;                       // LBO (unused for swizzled K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;               // SBO = 1024 B    [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                       // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                       // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                       // SWIZZLE_128B    [62,64)
   return d;
 }
-// Instruction descriptor, kind::f16: bf16 x bf16 -> fp32, both K-major.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t m, uint32_t n) {
-  return (1u << 4)      // D format  = F32
-       | (1u << 7)      // A format  = BF16
-       | (1u << 10)     // B format  = BF16
-       | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-// kind::f8f6f4 with e4m3 x e4m3 -> fp32 (format code 0 for both).
-__host__ __device__ constexpr uint32_t make_idesc_e4m3(uint32_t m, uint32_t n) {
-  return (1u << 4) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-
-// kind::mxf8f6f4.block_scale, e4m3 x e4m3, UE8M0 scales: [4,6) b_sf_id, [23] scale format E8M0, [29,31) a_sf_id
-__host__ __device__ constexpr uint32_t make_idesc_mxf8(uint32_t m, uint32_t n) {
-  return ((n >> 3) << 17) | (1u << 23) | ((m >> 4) << 24);
+// MN-major 128B-swizzled operand (rows = K index, 128-byte rows of 64 contiguous N elements):
+// LBO = distance between 64-element N blocks, SBO = distance between 8-row K groups (1024 B).
+__device__ __forceinline__ uint64_t make_sw128_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
 }
 
 // ------------------------------------------------------------ cluster / DSMEM
@@ -282,6 +181,14 @@ __device__ __forceinline__ uint2 ld_dsmem_v2u32(uint32_t cluster_addr) {
   uint2 v;
   asm volatile("ld.shared::cluster.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(cluster_addr) : "memory");
   return v;
+}
+// arrive on the mbarrier at this shared-memory offset in CTA `cta_rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta_rank) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(mapa_smem(smem_u32(bar), cta_rank))
+               : "memory");
+}
+__device__ __forceinline__ void st_dsmem_v2(uint32_t cluster_addr, float a, float b) {
+  asm volatile("st.shared::cluster.v2.f32 [%0], {%1,%2};" ::"r"(cluster_addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ void st_dsmem_f32(uint32_t cluster_addr, float v) {
   asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(cluster_addr), "f"(v) : "memory");
@@ -318,8 +225,8 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   return t;
 }
 
-// Slow path of a flag wait: out of line on purpose -- the decode GEMMs are sensitive to their code size (a bisect in
-// round 2 attributed 1-2 % of the step to a few hundred extra SASS instructions per kernel), and this is inlined nowhere.
+// Slow path of a flag wait: out of line on purpose -- the decode GEMMs are sensitive to their code size, and this is
+// inlined nowhere.
 static __device__ __noinline__ void wait_flag_slow(const uint32_t* flag, uint32_t target) {
   volatile uint32_t* ab = g_abort_word;
   if (ab != nullptr && *ab != 0u) return;                                        // mesh aborted: drain

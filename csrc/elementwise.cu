@@ -1,4 +1,4 @@
-// Bandwidth-bound helper kernels for sm_100a: RMSNorm / LayerNorm, embedding gather
+// Bandwidth-bound helper kernels for sm_90a: RMSNorm / LayerNorm, embedding gather
 // (optionally gated on the sampled-token flag written by the last piece over NVLink),
 // KV append for the unfused path, per-token 1/rms.  All 128-bit vectorised.
 // Reference parity: the ATen elementwise calls under bee2bee/hf.py:42-43.
@@ -234,7 +234,7 @@ __global__ void quant_fp8_rows_kernel(const __nv_bfloat16* __restrict__ x, uint8
 
 // MX (block-scaled) e4m3 quantisation of GEMM activations: one UE8M0 scale (2^e) per 32 consecutive K
 // elements, q = x * rstd * 2^-e.  Scale bytes are written directly in the 512-byte chunk layout that
-// tcgen05.cp expects for a token tile of `bn` rows (see GemmParams::sfb).  One CTA per token; a warp
+// GEMM expects for a token tile of `bn` rows (see GemmParams::sfb).  One CTA per token; a warp
 // iteration covers 128 K elements (8 lanes x 4 elements = one 32-element block).  Padding rows of the last
 // tile get scale 2^0 (a 0xFF byte would be NaN).
 // with_rms: 0 = plain, 1 = 1/rms folded into the values before quantisation, 2 = values quantised as they are and the

@@ -1,5 +1,5 @@
-// Fused GEMM epilogue math shared by the tcgen05 kernels: applied to 16 consecutive token
-// columns of one TMEM lane (= one output feature) after the accumulators have been read.
+// Fused GEMM epilogue math shared by the tensor-core kernels: applied to 16 consecutive token
+// columns of one output feature after the accumulators have been read.
 #pragma once
 #include "common.cuh"
 #include "gemm_tc.cuh"

@@ -1,25 +1,22 @@
-// tcgen05 / TMEM / TMA "swap-AB" GEMM for sm_100a.
+// wgmma / TMA "swap-AB" GEMM for sm_90a.
 //
 //   out[t, n] = epilogue( sum_k X[t, k] * W[n, k] )
 //
-// The WEIGHT matrix is the 128-row MMA "A" operand (UMMA_M = 128 output features
-// per CTA, one TMEM lane per feature) and the TOKENS are the MMA "N" dimension
-// (BN = 16..256 TMEM columns).  Decode batches of 1..32 tokens therefore cost
-// 16..32 tensor-core columns instead of a padded 128-row tile, the kernel streams
-// W exactly once through a TMA -> smem ring, and the whole op sits on the HBM
-// roofline.  Small problems get their parallelism from split-K across a
-// thread-block cluster whose partial accumulators are reduced through DSMEM.
+// The WEIGHT matrix is the 128-row MMA "A" operand (128 output features per CTA: two consumer warpgroups of
+// 64 rows, one m64 wgmma each) and the TOKENS are the MMA "N" dimension (BN = 16..256).  Decode batches of
+// 1..32 tokens therefore cost 16..32 tensor-core columns instead of a padded 128-row tile, the kernel streams
+// W exactly once through a TMA -> smem ring, and the whole op sits on the HBM roofline.  Small problems get
+// their parallelism from split-K across a thread-block cluster whose partial accumulators are reduced through
+// DSMEM.
 //
-// Roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer,
-// warps 2..5 = epilogue (TMEM -> registers -> fused epilogue -> global / peer).
+// Roles (288 threads): warps 0..7 = two consumer warpgroups (prologue, wgmma main loop, accumulators -> shared
+// memory), warp 8 = TMA producer; warps 0..3 then run the fused epilogue, one weight row per thread.
 //
-// Fused epilogues: residual add, SwiGLU/GeGLU, bias+GELU, RMSNorm scale of the
-// *input* (gamma folded into W; per-token 1/rms computed by the idle epilogue
-// warps during the main loop), RoPE + paged-KV append for the QKV projection,
-// and the NVLink piece handoff: the tail GEMM of piece i stores its tiles straight
-// into piece i+1's input buffer on the peer GPU and publishes a release flag; the
-// head GEMM of piece i+1 prefetches its weight tiles, acquires the flag, then
-// TMA-loads the freshly written activations.
+// Fused epilogues: residual add, SwiGLU/GeGLU, bias+GELU, RMSNorm scale of the *input* (gamma folded into W;
+// per-token 1/rms computed by the consumer warps while the producer fills the ring), RoPE + paged-KV append for
+// the QKV projection, and the NVLink piece handoff: the tail GEMM of piece i stores its tiles straight into
+// piece i+1's input buffer on the peer GPU and publishes a release flag; the head GEMM of piece i+1 prefetches
+// its weight tiles, acquires the flag, then TMA-loads the freshly written activations.
 //
 // Reference parity: replaces the JSON/WebSocket hidden-state hop of
 // bee2bee/node.py:249-277 and the cuBLAS calls under bee2bee/hf.py:42-43.
@@ -34,27 +31,34 @@
 
 #include "common.cuh"
 #include "launch.cuh"
+#include "wgmma.cuh"
 
 namespace b2b {
 
-constexpr int BM = 128;   // weight rows per CTA == UMMA_M
+constexpr int BM = 128;   // weight rows per CTA (two m64 warpgroups)
 constexpr int BK = 64;    // bf16 elements per 128B swizzle row (fp8: 128 elements, same 128 bytes)
 constexpr int ROW_BYTES = 128;
 constexpr int A_STAGE_BYTES = BM * ROW_BYTES;
+constexpr int GEMM_CONSUMERS = 256;                 // warps 0..7
+constexpr int GEMM_THREADS = GEMM_CONSUMERS + 32;   // + producer warp
 
 template <int BN>
 struct GemmCfg {
   static constexpr int kStages = (BN <= 32) ? 5 : (BN == 64 ? 4 : (BN == 128 ? 6 : 4));
   static constexpr int kStageBytes = A_STAGE_BYTES + BN * ROW_BYTES;
-  static constexpr int kTmemCols = BN < 32 ? 32 : BN;
-  // MX (block-scaled fp8): the UE8M0 scale factors of a stage (one 512-byte chunk per 128 rows x 128 K)
-  // are staged in smem next to the ring and copied to TMEM columns behind the accumulator.
+  // MX (block-scaled fp8): the UE8M0 scale factors of a stage (one 512-byte chunk per 128 rows x 128 K) are staged
+  // in smem next to the ring and applied per 32-K block to the partial products in registers.
   static constexpr int kSfaBytes = 512;
   static constexpr int kSfbBytes = BN > 128 ? 1024 : 512;
   static constexpr int kSfBytes = kSfaBytes + kSfbBytes;
-  static constexpr int kSfCol = kTmemCols;                      // first scale-factor column (2 x 16 columns)
-  static constexpr int kTmemColsMx = BN <= 32 ? 64 : (BN == 64 ? 128 : (BN == 128 ? 256 : 512));
-  static constexpr int smem_bytes(int stages) { return stages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/ + BN * 12 + stages * kSfBytes; }
+  // accumulators staged for the epilogue (128 rows x (BN + 4) fp32) + GLU exchange buffer; reuses the idle ring
+  static constexpr int kAccBytes = BM * (BN + 4) * 4 + BN * 256;
+  __host__ __device__ static constexpr int ring_bytes(int stages) {
+    return stages * kStageBytes > kAccBytes ? stages * kStageBytes : kAccBytes;
+  }
+  __host__ __device__ static constexpr int smem_bytes(int stages) {
+    return ring_bytes(stages) + 1024 /*align*/ + 256 /*barriers*/ + BN * 12 + stages * kSfBytes;
+  }
   static constexpr int kSmemBytes = smem_bytes(kStages);
 };
 
@@ -77,16 +81,17 @@ __device__ __forceinline__ unsigned long long gtime() {
   } while (0)
 
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 2, 256;" ::: "memory"); }
+__device__ __forceinline__ float ue8m0(uint8_t e) { return __uint_as_float(static_cast<uint32_t>(e) << 23); }
 
 // QM: 0 = bf16, 1 = fp8 e4m3 with per-row / per-token fp32 scales, 2 = MX fp8 (e4m3 + UE8M0 scale per 32 K)
-// MC: EXPERIMENTAL, untested on hardware in round 1 (default 1 = off).  MC > 1 launches clusters of MC CTAs along the
-//     weight-tile axis; the CTAs share one token tile, each TMA-loads 1/MC of it with `.multicast::cluster` into every
-//     CTA's stage, and a stage is released by all MC consumers (multicast tcgen05.commit).  Cuts the L2 -> SM traffic of the
-//     L2-bound prefill GEMM (profiles/rooflines.md) by up to 2x at MC = 4.
+// MC: (default 1 = off) MC > 1 launches clusters of MC CTAs along the weight-tile axis; the CTAs share one token tile,
+//     each TMA-loads 1/MC of it with `.multicast::cluster` into every CTA's stage, and a stage is released by the
+//     consumer warps of all MC CTAs.
 template <int BN, int EPI, int QM, int MC = 1>
-__global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w,
-                                                      const __grid_constant__ CUtensorMap tmap_x,
-                                                      const GemmParams p) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_w,
+                                                                  const __grid_constant__ CUtensorMap tmap_x,
+                                                                  const GemmParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr bool FP8 = QM != 0;
   constexpr bool MX = QM == 2;
@@ -96,18 +101,16 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
   const int STAGES = p.stages;            // ring depth (runtime: 2..Cfg::kStages; fewer stages = more CTAs per SM)
   constexpr int STAGE_BYTES = Cfg::kStageBytes;
   constexpr uint32_t TX_BYTES = STAGE_BYTES + (MX ? Cfg::kSfBytes : 0);
-  constexpr uint32_t TCOLS = MX ? Cfg::kTmemColsMx : Cfg::kTmemCols;
+  const int RING = Cfg::ring_bytes(STAGES);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + RING);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr_s = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-  float* rstd_s = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + 256);
+  float* rstd_s = reinterpret_cast<float*>(smem + RING + 256);
   int* pos_s = reinterpret_cast<int*>(rstd_s + BN);               // [BN] token positions (QKV/RoPE epilogue)
   int* slot_s = pos_s + BN;                                       // [BN] KV-cache slots
-  uint8_t* sf_s = smem + STAGES * STAGE_BYTES + 256 + BN * 12;    // [STAGES][kSfBytes]: SFA chunk, SFB chunk(s)
+  uint8_t* sf_s = smem + RING + 256 + BN * 12;                    // [STAGES][kSfBytes]: SFA chunk, SFB chunk(s)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -116,7 +119,6 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
   const int tok0 = blockIdx.y * BN;          // first token of this CTA
   const int splitk = p.splitk;
   const int krank = (splitk > 1) ? static_cast<int>(cluster_ctarank()) : 0;
-  const bool leader = (krank == 0);
   // split-K reduce-scatter: this CTA finishes token columns [col0, col0 + ncol) of the tile (launcher: splitk | BN)
   const int ncol = BN / splitk;
   const int col0 = krank * ncol;
@@ -127,26 +129,16 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
   const int kb_end = static_cast<int>((static_cast<long long>(nkb_total) * (krank + 1)) / splitk);
   const int nkb = kb_end - kb_begin;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == GEMM_CONSUMERS) {
     tma_prefetch_desc(&tmap_w);
     tma_prefetch_desc(&tmap_x);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&empty_bar[s], MCAST ? MC : 1);     // multicast: every consumer of the cluster releases the stage
-      }
-      mbar_init(tmem_full_bar, 1);
-      fence_barrier_init();
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8 * MC);     // every consumer warp of every CTA that reads the stage releases it
     }
-    __syncwarp();
-    tmem_alloc<TCOLS>(tmem_ptr_s);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_s;
   uint32_t crank = 0;
   if constexpr (MCAST) {
     // peers will multicast into this CTA's ring and arrive on its mbarriers: everyone's barriers must be initialised
@@ -158,7 +150,11 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
   pdl_launch_dependents();     // the next kernel may start its own set-up / weight prefetch now
   if (threadIdx.x == 0) B2B_DBG(1);
 
-  if (warp == 0) {
+  // split-K landing zone [splitk][128 rows][CW + 4] and GLU exchange buffer [ncol][64] behind it: both reuse the ring
+  float* red = reinterpret_cast<float*>(smem);
+  const int CWP = ncol + 4;                      // row pitch in floats (16-byte aligned rows, bank spread)
+
+  if (warp == GEMM_CONSUMERS / 32) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
       const uint64_t pol_w = l2_policy_evict_first();   // weights: streamed once
@@ -184,8 +180,8 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
           tma_load_2d_multicast(smem + i * STAGE_BYTES + A_STAGE_BYTES + crank * (BN / MC) * ROW_BYTES, &tmap_x, &full_bar[i],
                                 (kb_begin + i) * BKE, tok0 + static_cast<int>(crank) * (BN / MC), MC_MASK);
         else
-        tma_load_2d_hint(smem + i * STAGE_BYTES + A_STAGE_BYTES, &tmap_x, &full_bar[i], (kb_begin + i) * BKE, tok0,
-                         pol_x);
+          tma_load_2d_hint(smem + i * STAGE_BYTES + A_STAGE_BYTES, &tmap_x, &full_bar[i], (kb_begin + i) * BKE, tok0,
+                           pol_x);
         if constexpr (MX)
           bulk_load(sf_s + i * Cfg::kSfBytes + Cfg::kSfaBytes, sfb_g + static_cast<size_t>(i) * Cfg::kSfbBytes, Cfg::kSfbBytes, &full_bar[i]);
       }
@@ -202,8 +198,8 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
           tma_load_2d_multicast(smem + s * STAGE_BYTES + A_STAGE_BYTES + crank * (BN / MC) * ROW_BYTES, &tmap_x, &full_bar[s],
                                 (kb_begin + kb) * BKE, tok0 + static_cast<int>(crank) * (BN / MC), MC_MASK);
         else
-        tma_load_2d_hint(smem + s * STAGE_BYTES + A_STAGE_BYTES, &tmap_x, &full_bar[s],
-                         (kb_begin + kb) * BKE, tok0, pol_x);
+          tma_load_2d_hint(smem + s * STAGE_BYTES + A_STAGE_BYTES, &tmap_x, &full_bar[s],
+                           (kb_begin + kb) * BKE, tok0, pol_x);
         if constexpr (MX) {
           bulk_load(sf_s + s * Cfg::kSfBytes, sfa_g + static_cast<size_t>(kb) * Cfg::kSfaBytes, Cfg::kSfaBytes, &full_bar[s]);
           bulk_load(sf_s + s * Cfg::kSfBytes + Cfg::kSfaBytes, sfb_g + static_cast<size_t>(kb) * Cfg::kSfbBytes, Cfg::kSfbBytes, &full_bar[s]);
@@ -211,57 +207,23 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // -------------------------------------------------------------- MMA issuer
-    constexpr uint32_t idesc = MX ? make_idesc_mxf8(BM, BN) : (FP8 ? make_idesc_e4m3(BM, BN) : make_idesc_bf16(BM, BN));
-    int s = 0;
-    uint32_t ph = 0;
-    for (int kb = 0; kb < nkb; ++kb) {
-      mbar_wait(&full_bar[s], ph);
-      tc_fence_after();
-      if (lane == 0) {
-        if (kb == 0) B2B_DBG(3);
-        const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(smem + s * STAGE_BYTES));
-        const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(smem + s * STAGE_BYTES + A_STAGE_BYTES));
-        uint32_t sfa_t = 0, sfb_t = 0;
-        if constexpr (MX) {
-          // scale factors of this stage: smem -> TMEM (tcgen05.cp executes in issue order with the MMAs below);
-          // two column sets alternate so that the copy for stage kb+1 never races the MMAs of stage kb
-          sfa_t = tmem_base + Cfg::kSfCol + static_cast<uint32_t>(kb & 1) * 16;
-          sfb_t = sfa_t + 4;
-          const uint32_t sf_addr = smem_u32(sf_s + s * Cfg::kSfBytes);
-          tmem_cp_32x128b_warpx4(sfa_t, make_sf_desc(sf_addr));
-          tmem_cp_32x128b_warpx4(sfb_t, make_sf_desc(sf_addr + Cfg::kSfaBytes));
-          if constexpr (BN > 128) tmem_cp_32x128b_warpx4(sfb_t + 4, make_sf_desc(sf_addr + Cfg::kSfaBytes + 512));
-        }
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          // advance 16 bf16 = 32 B along K inside the swizzle atom: +2 in the (addr>>4) field
-          // one MMA consumes 32 bytes of K per row (16 bf16 / 32 e4m3): +2 in the (addr >> 4) field
-          if constexpr (MX)
-            umma_mxf8(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc | (static_cast<uint32_t>(k) << 4) | (static_cast<uint32_t>(k) << 29),
-                      (kb > 0 || k > 0) ? 1u : 0u, sfa_t, sfb_t);
-          else if constexpr (FP8) umma_f8(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          else umma_bf16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-        }
-        if constexpr (MCAST) umma_commit_multicast(&empty_bar[s], MC_MASK);   // every producer of the cluster writes this slot
-        else umma_commit(&empty_bar[s]);               // frees the smem slot when the MMAs retire
-        if (kb == nkb - 1) { umma_commit(tmem_full_bar); B2B_DBG(4); }   // accumulator complete
-      }
-      __syncwarp();
-      if (++s == STAGES) { s = 0; ph ^= 1; }
+    // split-K: the consumers pass two cluster barriers (ring idle, partials scattered); the producer warp takes part in
+    // the first here and in the second below, so every thread of the cluster arrives at both
+    if (splitk > 1) {
+      cluster_arrive_release();
+      cluster_wait_acquire();
     }
   } else {
-    // ---------------------------------------- epilogue warps: prologue work
+    // ---------------------------------------- consumer warps: prologue work
     // Every CTA of a split-K cluster finishes its own slice of token columns [col0, col0 + ncol)
     // (reduce-scatter, see below), so each CTA only needs the per-token inputs of that slice.
-    const int et = threadIdx.x - 64;   // 0..127
+    const int et = threadIdx.x;        // 0..255
     pdl_wait();                        // everything below reads / writes memory of earlier kernels
     {
       if constexpr (EPI == EPI_QKV_ROPE) {
         // per-token metadata -> smem once: global loads inside the store loop of the epilogue serialise on L2
-        // latency (the compiler cannot hoist them above stores that may alias): +8 us at 32 tokens
-        for (int t = col0 + et; t < col0 + ncol; t += 128) {
+        // latency (the compiler cannot hoist them above stores that may alias)
+        for (int t = col0 + et; t < col0 + ncol; t += GEMM_CONSUMERS) {
           const int tok = tok0 + t;
           pos_s[t] = (p.positions != nullptr && tok < p.m_tok) ? p.positions[tok] : 0;
           slot_s[t] = (tok < p.m_tok) ? p.slots[tok] : -1;
@@ -274,15 +236,16 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
         }
         // one warp per token, FOUR tokens x FOUR row segments in flight per lane (the loop is L2-latency
         // bound: 16 independent 128-bit loads are issued before the first use)
+        constexpr int NW = GEMM_CONSUMERS / 32;
         const int kv8 = p.k / 8;
-        for (int tr = warp - 2; tr < ncol; tr += 16) {
+        for (int tr = warp; tr < ncol; tr += 4 * NW) {
           float ss[4] = {0.f, 0.f, 0.f, 0.f};
           const uint4* rowp[4];
           bool live[4];
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
-            const int tok = tok0 + col0 + tr + 4 * u;
-            live[u] = (tr + 4 * u < ncol) && tok < p.m_tok;
+            const int tok = tok0 + col0 + tr + NW * u;
+            live[u] = (tr + NW * u < ncol) && tok < p.m_tok;
             rowp[u] = reinterpret_cast<const uint4*>(p.norm_src + static_cast<size_t>(live[u] ? tok : tok0) * p.k);
           }
           for (int i0 = lane; i0 < kv8; i0 += 128) {
@@ -308,8 +271,8 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
           for (int u = 0; u < 4; ++u) {
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) ss[u] += __shfl_xor_sync(0xffffffffu, ss[u], o);
-            if (lane == 0 && tr + 4 * u < ncol)
-              rstd_s[col0 + tr + 4 * u] = live[u] ? rsqrtf(ss[u] / static_cast<float>(p.k) + p.eps) : 0.f;
+            if (lane == 0 && tr + NW * u < ncol)
+              rstd_s[col0 + tr + NW * u] = live[u] ? rsqrtf(ss[u] / static_cast<float>(p.k) + p.eps) : 0.f;
           }
         }
       } else {
@@ -320,7 +283,7 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
             wait_flag_ge(p.wait_flag, target);
           }
         }
-        for (int t = col0 + et; t < col0 + ncol; t += 128) {
+        for (int t = col0 + et; t < col0 + ncol; t += GEMM_CONSUMERS) {
           const int tok = tok0 + t;
           float r = (p.rstd != nullptr && tok < p.m_tok) ? p.rstd[tok] : 1.f;
           if constexpr (MX) {
@@ -331,66 +294,142 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
         }
         if constexpr (MX) {
           if (p.zero_buf != nullptr && blockIdx.x == 0 && blockIdx.z == 0)
-            for (int t = et; t < BN; t += 128)
+            for (int t = et; t < BN; t += GEMM_CONSUMERS)
               if (tok0 + t < p.m_tok) p.zero_buf[tok0 + t] = 0.f;
         }
       }
-      epi_bar_sync();
     }
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    if (threadIdx.x == 64) B2B_DBG(5);
-  }
 
-  // ------------------------------------- split-K reduce-scatter through DSMEM
-  // After barrier #1 every CTA's main loop has retired, so all stage rings are free.  CTA r of the cluster owns
-  // the token columns [r*CW, (r+1)*CW): every CTA scatters its partial accumulator column slices into the owners'
-  // landing zones (its own slice included), barrier #2, then every CTA adds the `splitk` partials of its slice and
-  // runs the fused epilogue for those CW tokens only.  Compared with "everything to the leader" the epilogue work
-  // (residual / RoPE / stores) is spread over the cluster and no CTA idles.
-  const int q = warp & 3;
-  const int row = q * 32 + lane;                 // TMEM lane == weight row within the tile
-  const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-  float* red = reinterpret_cast<float*>(smem);   // landing zone [splitk][128 rows][CW + 4]
-  const int CWP = ncol + 4;                      // row pitch in floats (16-byte aligned rows, bank spread)
-  if (splitk > 1) {
-    cluster_arrive_release();
-    cluster_wait_acquire();
-    if (warp >= 2) {
-      const uint32_t zone = smem_u32(red) + static_cast<uint32_t>(((krank * BM + row) * CWP) * 4);
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 16) {
-        float v[16];
-        tmem_ld16(taddr + c, v);
-        if (ncol >= 4) {
+    // -------------------------------------------------------------- wgmma main loop
+    const int wg = warp >> 2;                                     // rows [64 wg, 64 wg + 64) of the weight tile
+    float acc[BN / 2];
 #pragma unroll
-          for (int i = 0; i < 16; i += 4) {
-            const int col = c + i, d = col / ncol, off = col - d * ncol;
-            st_dsmem_v4(mapa_smem(zone, static_cast<uint32_t>(d)) + static_cast<uint32_t>(off * 4),
-                        make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]));
-          }
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) {
+        if constexpr (MCAST) {
+#pragma unroll
+          for (int c = 0; c < MC; ++c) mbar_arrive_cluster(&empty_bar[s], static_cast<uint32_t>(c));
         } else {
+          mbar_arrive(&empty_bar[s]);
+        }
+      }
+    };
+    int s = 0, prev = -1;
+    uint32_t ph = 0;
+    for (int kb = 0; kb < nkb; ++kb) {
+      mbar_wait(&full_bar[s], ph);
+      if (threadIdx.x == 0 && kb == 0) B2B_DBG(3);
+      const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(smem + s * STAGE_BYTES + wg * 64 * ROW_BYTES));
+      const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(smem + s * STAGE_BYTES + A_STAGE_BYTES));
+      if constexpr (MX) {
+        // one e4m3 wgmma per 32-K block (= one UE8M0 scale) into a partial tile, scaled into the accumulators:
+        // acc[r][c] += 2^(sfa[r]) * 2^(sfb[c]) * partial[r][c]
+        constexpr int NC = BN < 128 ? BN : 128;
+        const uint8_t* sfa = sf_s + s * Cfg::kSfBytes;
+        const uint8_t* sfb = sfa + Cfg::kSfaBytes;
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int col = c + i, d = col / ncol, off = col - d * ncol;
-            st_dsmem_f32(mapa_smem(zone, static_cast<uint32_t>(d)) + static_cast<uint32_t>(off * 4), v[i]);
+        for (int j = 0; j < 4; ++j) {
+          const float sa0 = ue8m0(sfa[(r0 & 31) * 16 + (r0 >> 5) * 4 + j]);
+          const float sa1 = ue8m0(sfa[((r0 + 8) & 31) * 16 + ((r0 + 8) >> 5) * 4 + j]);
+#pragma unroll
+          for (int h = 0; h < BN / NC; ++h) {
+            float part[NC / 2];
+#pragma unroll
+            for (int i = 0; i < NC / 2; ++i) part[i] = 0.f;
+            wgmma_fence();
+            Wgmma<NC>::e4m3_ss(part, adesc + 2 * j, bdesc + static_cast<uint64_t>(h * NC * ROW_BYTES / 16) + 2 * j, 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(part);
+#pragma unroll
+            for (int jj = 0; jj < NC / 8; ++jj) {
+              const int c = h * NC + jj * 8 + 2 * (lane & 3);
+              const int cr = c & 127, cr1 = (c + 1) & 127;
+              const float sb0 = ue8m0(sfb[(c >> 7) * 512 + (cr & 31) * 16 + (cr >> 5) * 4 + j]);
+              const float sb1 = ue8m0(sfb[((c + 1) >> 7) * 512 + (cr1 & 31) * 16 + (cr1 >> 5) * 4 + j]);
+              float* a = acc + h * (NC / 2) + 4 * jj;
+              a[0] = fmaf(part[4 * jj + 0], sa0 * sb0, a[0]);
+              a[1] = fmaf(part[4 * jj + 1], sa0 * sb1, a[1]);
+              a[2] = fmaf(part[4 * jj + 2], sa1 * sb0, a[2]);
+              a[3] = fmaf(part[4 * jj + 3], sa1 * sb1, a[3]);
+            }
           }
+        }
+        release(s);
+      } else {
+        wgmma_fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          // one MMA consumes 32 bytes of K per row (16 bf16 / 32 e4m3): +2 in the (addr >> 4) field
+          if constexpr (FP8) Wgmma<BN>::e4m3_ss(acc, adesc + 2 * k, bdesc + 2 * k, (kb > 0 || k > 0) ? 1u : 0u);
+          else Wgmma<BN>::bf16_ss(acc, adesc + 2 * k, bdesc + 2 * k, (kb > 0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();             // the MMAs of the previous stage have retired: hand its slot back
+        wgmma_fence_regs(acc);
+        if (prev >= 0) release(prev);
+        prev = s;
+      }
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+    if constexpr (!MX) {
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0) release(prev);
+    }
+    if (threadIdx.x == 0) B2B_DBG(4);
+
+    // ---------------------------------------- accumulators -> landing zone(s)
+    // Every CTA's ring must be idle before it is overwritten: the consumers of this CTA (and, for split-K, of the
+    // whole cluster) have retired their MMAs at the barrier below.
+    if (splitk > 1) {
+      cluster_arrive_release();
+      cluster_wait_acquire();
+    } else {
+      consumer_bar_sync();
+    }
+    // CTA r of the cluster owns the token columns [r*CW, (r+1)*CW): every CTA scatters its partial accumulator column
+    // slices into the owners' landing zones (its own slice included), barrier, then every CTA adds the `splitk`
+    // partials of its slice and runs the fused epilogue for those CW tokens only.
+    const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int jj = 0; jj < BN / 8; ++jj) {
+      const int col = jj * 8 + 2 * (lane & 3);          // even; ncol is even, so (col, col + 1) share an owner
+      const int d = col / ncol, off = col - d * ncol;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = rbase + 8 * hh;
+        const float v0 = acc[4 * jj + 2 * hh], v1 = acc[4 * jj + 2 * hh + 1];
+        if (splitk > 1) {
+          const uint32_t a = smem_u32(red) + static_cast<uint32_t>(((krank * BM + row) * CWP + off) * 4);
+          st_dsmem_v2(mapa_smem(a, static_cast<uint32_t>(d)), v0, v1);
+        } else {
+          *reinterpret_cast<float2*>(red + row * CWP + off) = make_float2(v0, v1);
         }
       }
     }
+  }
+
+  if (splitk > 1) {
     cluster_arrive_release();
     cluster_wait_acquire();
+  } else {
+    __syncthreads();
   }
 
   // ------------------------------------------------------------ fused epilogue
-  if (warp >= 2) {
+  if (warp < 4) {
+    const int row = threadIdx.x;                 // weight row within the tile
     const int n_glob = tile_n * BM + row;
-    float* xch = red + (splitk > 1 ? splitk * BM * CWP : 0);   // GLU exchange buffer [ncol][64] (behind the landing zone, if any)
+    float* xch = red + splitk * BM * CWP;        // GLU exchange buffer [ncol][64] (behind the landing zone)
     const float bias_v = (p.bias != nullptr) ? p.bias[n_glob] : 0.f;
     // fp8: per-output-row weight scale (the per-token activation scale rides in rstd_s)
     const float wsc = (FP8 && p.w_scale != nullptr) ? p.w_scale[n_glob] : 1.f;
     const float wsc_up = (FP8 && EPI == EPI_GLU && p.w_scale != nullptr && row < 64) ? p.w_scale[n_glob + 64] : 1.f;
-
     if (p.free_flag != nullptr) {
       // back-pressure: the consumer must have drained the previous payload of this slot
       const uint32_t e = *reinterpret_cast<const volatile uint32_t*>(p.signal_epoch);
@@ -466,9 +505,7 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
 
     // accumulators of up to 16 columns starting at local column c (slice-relative)
     auto load_acc = [&](int c, int n, float* v) {
-      if (splitk == 1) {
-        tmem_ld16(taddr + c, v);
-      } else {
+      {
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] = 0.f;
         for (int r = 0; r < splitk; ++r) {
@@ -545,7 +582,7 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
           reinterpret_cast<__nv_bfloat16*>(p.out)[static_cast<size_t>(tok) * p.ld_out + n_glob] = r16;
           if (p.out2 != nullptr)
             reinterpret_cast<__nv_bfloat16*>(p.out2)[static_cast<size_t>(tok) * p.ld_out + n_glob] = r16;
-          if constexpr (MX) {      // (anything of the fused quantiser left in the bf16 instantiations cost 50 us per step)
+          if constexpr (MX) {      // (kept out of the bf16 instantiations: the decode GEMMs are sensitive to code size)
             qv[i] = rv;
             q_valid = i + 1;
           }
@@ -583,12 +620,12 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
       }
     }
 
-    if (threadIdx.x == 64) B2B_DBG(6);
+    if (threadIdx.x == 0) B2B_DBG(6);
     // ------------------------------------------------ handoff publication
     if (p.signal_flag != nullptr || p.bump_epoch != nullptr) {
       __threadfence_system();            // my (possibly peer-directed) stores are performed
       epi_bar_sync();
-      if (threadIdx.x == 64) {
+      if (threadIdx.x == 0) {
         const uint32_t total = gridDim.x * gridDim.y * gridDim.z;   // every CTA of a split-K cluster stores a slice
         const uint32_t prev = atomicAdd(p.done_counter, 1u);
         if (prev == total - 1) {
@@ -613,12 +650,6 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
     // no CTA may leave while a peer can still multicast into its ring or arrive on its barriers
     cluster_arrive_release();
     cluster_wait_acquire();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<TCOLS>(tmem_base);
   }
   if (threadIdx.x == 0) B2B_DBG(7);
 }
@@ -685,10 +716,10 @@ static int launch_bn_epi(const GemmParams& p, const CUtensorMap& tw, const CUten
     if (dev < 64) attr_set[dev] = true;
   }
   return static_cast<int>(launch_kernel(gemm_tc_kernel<BN, EPI, QM>, dim3(p.n_out / BM, (p.m_tok + BN - 1) / BN, p.splitk),
-                                        dim3(192), Cfg::smem_bytes(p.stages), stream, static_cast<unsigned>(p.splitk), tw, tx, p));
+                                        dim3(GEMM_THREADS), Cfg::smem_bytes(p.stages), stream, static_cast<unsigned>(p.splitk), tw, tx, p));
 }
 
-// EXPERIMENTAL multicast launch (bf16, token tiles of 128 / 256, no split-K): cluster of MC CTAs along grid.x
+// multicast launch (bf16, token tiles of 128 / 256, no split-K): cluster of MC CTAs along grid.x
 template <int BN, int EPI, int MC>
 static int launch_mc(const GemmParams& p, const CUtensorMap& tw, const CUtensorMap& tx_slice, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
@@ -702,7 +733,7 @@ static int launch_mc(const GemmParams& p, const CUtensorMap& tw, const CUtensorM
     attr_set[dev] = true;
   }
   return static_cast<int>(launch_kernel_cx(gemm_tc_kernel<BN, EPI, 0, MC>, dim3(p.n_out / BM, (p.m_tok + BN - 1) / BN, 1),
-                                           dim3(192), Cfg::smem_bytes(p.stages), stream, static_cast<unsigned>(MC), tw, tx_slice, p));
+                                           dim3(GEMM_THREADS), Cfg::smem_bytes(p.stages), stream, static_cast<unsigned>(MC), tw, tx_slice, p));
 }
 template <int BN, int MC>
 static int launch_mc_epi(const GemmParams& p, const CUtensorMap& tw, const CUtensorMap& tx_slice, cudaStream_t stream) {
@@ -716,8 +747,8 @@ static int launch_mc_epi(const GemmParams& p, const CUtensorMap& tw, const CUten
   }
 }
 
-// one compact kernel per (token tile, epilogue): a runtime `switch` in the 16x-unrolled epilogue
-// loop made the kernel instruction-fetch bound (5.4 us epilogue, see profiles/gemm_timeline.md)
+// one compact kernel per (token tile, epilogue): a runtime `switch` inside the 16x-unrolled epilogue
+// loop would make the kernel instruction-fetch bound
 template <int BN>
 static int launch_bn(const GemmParams& p, const CUtensorMap& tw, const CUtensorMap& tx, cudaStream_t stream) {
 #define B2B_EPI_CASE(E)                                                                              \
@@ -782,20 +813,21 @@ int gemm_tc_default_stages(int bn) {
 
 int gemm_tc_max_splitk(int bn, int epi, int stages) {
   // reduce-scatter landing zone in every CTA's stage ring: S * 128 rows * (BN/S + 4) floats (+ GLU exchange BN/S * 256 B)
-  int stage_bytes;
+  int ring;
   const int dflt = gemm_tc_default_stages(bn);
   if (stages <= 0 || stages > dflt) stages = dflt;
+  if (stages < 2) stages = 2;
   switch (bn) {
-    case 16: stage_bytes = GemmCfg<16>::kStageBytes; break;
-    case 32: stage_bytes = GemmCfg<32>::kStageBytes; break;
-    case 64: stage_bytes = GemmCfg<64>::kStageBytes; break;
-    case 128: stage_bytes = GemmCfg<128>::kStageBytes; break;
-    default: stage_bytes = GemmCfg<256>::kStageBytes; break;
+    case 16: ring = GemmCfg<16>::ring_bytes(stages); break;
+    case 32: ring = GemmCfg<32>::ring_bytes(stages); break;
+    case 64: ring = GemmCfg<64>::ring_bytes(stages); break;
+    case 128: ring = GemmCfg<128>::ring_bytes(stages); break;
+    default: ring = GemmCfg<256>::ring_bytes(stages); break;
   }
   int best = 1;
   for (int s = 2; s <= 8 && bn / s >= 2; s *= 2) {
     const int need = s * 128 * (bn / s + 4) * 4 + (epi == EPI_GLU ? (bn / s) * 256 : 0);
-    if (need <= stages * stage_bytes) best = s;
+    if (need <= ring) best = s;
   }
   return best;
 }
@@ -811,13 +843,6 @@ int launch_gemm_tc(const GemmParams& p_in, const void* w, const void* x, int bn,
     const int dflt = gemm_tc_default_stages(bn);
     if (p.stages <= 0 || p.stages > dflt) p.stages = dflt;
     if (p.stages < 2) p.stages = 2;
-  }
-  {
-    // the epilogue reuses the (by then idle) stage ring: GLU exchange buffer bn x 64 floats when there is no split-K
-    // landing zone in front of it -- a shallow ring must still hold it
-    const int stage_bytes = 128 * 128 + bn * 128;
-    const int need = (p.epi == EPI_GLU) ? bn * 256 : 0;
-    while (p.stages * stage_bytes < need && p.stages < gemm_tc_default_stages(bn)) ++p.stages;
   }
   const int smax = gemm_tc_max_splitk(bn, p.epi, p.stages);
   if (p.splitk > smax) p.splitk = smax;

@@ -1,4 +1,4 @@
-// C launcher API of the hand-written sm_100a kernels (no torch dependency: every .cu
+// C launcher API of the hand-written sm_90a kernels (no torch dependency: every .cu
 // compiles in seconds with plain nvcc; csrc/binding.cpp is the only torch-facing file).
 #pragma once
 #include <cuda_runtime.h>
@@ -33,13 +33,13 @@ int launch_attention(const void* q, const void* k_cache, const void* v_cache, vo
                      int max_pages, int n_q, int n_kv, int head_dim, int window, float softcap, int splits,
                      cudaStream_t s);
 int attn_rows(int G, int QB);
-// attention_tc.cu: tcgen05 flash-attention forward for prefill chunks
+// attention_tc.cu: wgmma flash-attention forward for prefill chunks
 bool attention_tc_supported(int n_q, int n_kv, int head_dim);
 int launch_attention_tc(const void* q, const void* k_cache, const void* v_cache, void* out, const int* block_table,
                         const int* q_start, const int* q_len, const int* kv_len, int seqs, int max_q, int max_pages,
                         int n_tokens, int n_pages, int n_q, int n_kv, int head_dim, int window, float softcap,
                         int splits, float* ws, void* q_out8, void* q_sf, int q_bn, cudaStream_t s);
-// merge pass of split-KV decode (shared by the CUDA-core and the tcgen05 kernels)
+// merge pass of split-KV decode (shared by the CUDA-core and the tensor-core kernels)
 int launch_attention_merge(void* out, const int* q_start, const float* ws, int seqs, int n_q, int n_kv, int head_dim,
                            int splits, cudaStream_t s);
 int attention_init();

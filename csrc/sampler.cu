@@ -1,4 +1,4 @@
-// Fused sampler for sm_100a: repetition penalty (seen-token bitmap) -> temperature ->
+// Fused sampler for sm_90a: repetition penalty (seen-token bitmap) -> temperature ->
 // exact top-p via two-level radix histogram of the probability bits -> multinomial draw
 // (or argmax when temperature <= 0).  One CTA per sequence, logits are fp32 [B, ld] as
 // written by the lm_head GEMM.  The sampled id is stored locally (token ring, history
@@ -8,7 +8,7 @@
 // Semantics follow the reference's generation defaults (bee2bee/hf.py:91-105):
 // repetition_penalty 1.15, top_p 0.95, do_sample iff temperature > 0, greedy otherwise.
 //
-// Performance notes (profiles/launches_decode_step.md): every pass over the 128k logits is
+// Performance notes: every pass over the 128k logits is
 // L2-latency bound, so logits are read 8 at a time per thread (2 x 128-bit loads in flight);
 // histogram mass is accumulated in 32.32 fixed point with native 32-bit shared-memory atomics
 // (float / 64-bit shared atomics are CAS loops).
@@ -96,7 +96,7 @@ __device__ __forceinline__ void hist_add(uint32_t* lo, uint32_t* hi, int bin, ui
 }
 
 // One CLUSTER of CS CTAs per sequence (grid = [B, 1, CS]); CTA r owns ids [r*W, (r+1)*W).  A single
-// SM is instruction-bound on a 128k vocabulary (about 28 us per pass, profiles/bench_history.md), so the
+// SM is instruction-bound on a 128k vocabulary, so the
 // vocabulary is spread over CS SMs, each slice is read from L2 exactly once and then lives in shared
 // memory as exp(l - max); the per-level histograms are merged across the cluster through DSMEM.
 __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SampleParams p, const int W) {
@@ -455,12 +455,18 @@ int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* pee
   int cs = 1;
   while (cs < MAX_CS && (vocab + cs - 1) / cs > MAX_SLICE) cs *= 2;
   if ((vocab + cs - 1) / cs > MAX_SLICE) return -6;
-  while (cs < MAX_CS && batch * cs * 2 <= 148) cs *= 2;
+  static int sm_count[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  int sms = dev < 64 ? sm_count[dev] : 0;
+  if (sms == 0) {
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -9;
+    if (dev < 64) sm_count[dev] = sms;
+  }
+  while (cs < MAX_CS && batch * cs * 2 <= sms) cs *= 2;
   const int W = (((vocab + cs - 1) / cs) + 127) & ~127;
   const size_t smem = sizeof(SampShared) + static_cast<size_t>(W) * sizeof(float);
   static bool attr_set[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
   if (dev < 64 && !attr_set[dev]) {
     const cudaError_t e = cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                static_cast<int>(sizeof(SampShared) + MAX_SLICE * sizeof(float)));

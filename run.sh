@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Provider launcher (parity: /root/reference/run.sh): builds the sm_100a extension if needed, then
+# Provider launcher (parity: /root/reference/run.sh): builds the sm_90a extension if needed, then
 # serves MODEL through PROVIDER (hf | ollama | hf_remote) with PIECES layer pieces.
 set -euo pipefail
 MODEL="${MODEL:-distilgpt2}"; PROVIDER="${PROVIDER:-hf}"; PORT="${PORT:-0}"; API_PORT="${API_PORT:-8000}"; PIECES="${PIECES:-1}"

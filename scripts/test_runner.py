@@ -2,7 +2,7 @@
 import-smokes its test modules; this one actually runs them through pytest).
 
     python scripts/test_runner.py            # -m "not gpu"
-    python scripts/test_runner.py --gpu      # kernel / model / multi-GPU tiers on a B200 host
+    python scripts/test_runner.py --gpu      # kernel / model / multi-GPU tiers on a H100 host
 """
 import os
 import subprocess

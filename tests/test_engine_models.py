@@ -269,7 +269,7 @@ def test_piece_units_cover_the_model_and_balance_the_wavefront():
 
 
 def test_mx_block_scaled_quantisation_roundtrip_cpu():
-    """OCP-MX e4m3: one power-of-two scale per 32 K elements; chunk layout used by tcgen05.cp is a pure permutation."""
+    """OCP-MX e4m3: one power-of-two scale per 32 K elements; the GEMM's scale-factor chunk layout is a pure permutation."""
     from bee2bee_b200 import ops
 
     torch.manual_seed(0)
@@ -301,11 +301,11 @@ def test_split_k_heuristic_matches_the_measured_optimum():
     shapes = dict(qkv=(6144, 4096), o=(4096, 4096), gu=(28672, 4096), down=(4096, 14336), head=(128256, 4096))
     with mock.patch.object(ops, "native", lambda: fake):
         pick = lambda bn, m: {k: ops.pick_splitk(n, m, kk, bn, 0) for k, (n, kk) in shapes.items()}
-        assert pick(32, 32) == dict(qkv=4, o=4, gu=1, down=8, head=1)      # profiles/raw/layer_sweep_reduce_scatter.txt
+        assert pick(32, 32) == dict(qkv=4, o=4, gu=1, down=8, head=1)      # up to ~2 CTAs per SM
         assert pick(16, 1) == dict(qkv=4, o=4, gu=1, down=4, head=1)       # >= 4 token columns per CTA of the cluster
         assert all(v == 1 for v in pick(256, 4096).values())               # prefill: tiles already fill the machine
-    # prefill chunks: (token tile, ring depth, split-K) per GEMM of a Llama-3-8B layer (profiles/prefill_gemm.md, split-K
-    # sweep): under-filled GEMMs are split along K until the machine is full instead of running two waves
+    # prefill chunks: (token tile, ring depth, split-K) per GEMM of a Llama-3-8B layer: under-filled GEMMs are split
+    # along K until the machine is full instead of running two waves
     tile = lambda m: {k: ops.pick_prefill_tile(n, m, kk) for k, (n, kk) in shapes.items() if k != "head"}
     assert tile(512) == dict(qkv=(128, 3, 1), o=(128, 3, 2), gu=(256, 2, 1), down=(256, 0, 2))
     assert tile(256) == dict(qkv=(128, 3, 2), o=(128, 3, 2), gu=(128, 3, 1), down=(256, 0, 4))

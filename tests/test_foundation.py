@@ -178,7 +178,7 @@ def test_nat_api_is_inert_offline():
 
 
 def test_mesh_staging_plan_sizes_quantised_hop_buffers():
-    """fp8 across the handoff: the hop slots for the e4m3 stream, its scale-factor chunks (tcgen05.cp layout: 512 B per
+    """fp8 across the handoff: the hop slots for the e4m3 stream, its scale-factor chunks (chunk layout: 512 B per
     32-row tile and 128 K) and the sum-of-squares counters exist only for mxfp8 meshes; a gate/up | down cut adds the
     e4m3 MLP hidden.  (Pure sizing logic -- the buffers themselves are cudaMalloc + IPC, tests/test_multigpu.py.)"""
     import torch

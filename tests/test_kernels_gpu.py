@@ -1,4 +1,4 @@
-"""Numerics of every hand-written sm_100a kernel against a plain PyTorch fp32 reference."""
+"""Numerics of every hand-written sm_90a kernel against a plain PyTorch fp32 reference."""
 import math
 
 import os
@@ -229,7 +229,7 @@ def _attn_ref(q, kc, vc, bt, q_lens, kv_lens, nq, nkv, hd, window, softcap):
 @pytest.mark.parametrize("window,softcap", [(0, 0.0), (100, 50.0)])
 @pytest.mark.parametrize("use_tc", [1, 0])
 def test_attention_decode(hd, nq, nkv, window, softcap, use_tc):
-    """decode (one query token per sequence) on the tcgen05 flash kernel (one-token query blocks, the default) and on
+    """decode (one query token per sequence) on the tensor-core flash kernel (one-token query blocks, the default) and on
     the CUDA-core kernel; an inactive batch row (q_len 0) must be left alone by both"""
     kv_lens = [1, 63, 64, 65, 300, 17, 1000]
     S = len(kv_lens)
@@ -252,7 +252,7 @@ def test_attention_decode(hd, nq, nkv, window, softcap, use_tc):
 @pytest.mark.parametrize("use_tc", [1, 0])
 @pytest.mark.parametrize("hd,nq,nkv", [(128, 8, 2), (256, 8, 4)])
 def test_attention_decode_split_kv(splits, use_tc, hd, nq, nkv):
-    """split-KV decode: (sequence, kv head, split) CTAs + merge pass, on the tcgen05 kernel and the CUDA-core kernel;
+    """split-KV decode: (sequence, kv head, split) CTAs + merge pass, on the tensor-core kernel and the CUDA-core kernel;
     splits with no tiles at all (short sequences) publish empty partials"""
     kv_lens = [1000, 130, 64, 5]
     S = len(kv_lens)
@@ -310,7 +310,7 @@ def test_attention_prefill_scalar_fallback_kernel():
     (64, 12, 12, 0, 0.0),        # GPT-2: MHA, d=64
 ])
 def test_attention_prefill_tcgen05_long(hd, nq, nkv, window, softcap):
-    """tcgen05 flash-attention prefill: long prompts, chunked prefill on top of cached context, ragged batch."""
+    """tensor-core flash-attention prefill: long prompts, chunked prefill on top of cached context, ragged batch."""
     q_lens = [1000, 257, 640]
     kv_lens = [1000, 900, 640]         # sequence 1 is a second chunk on top of 643 cached tokens
     kc, vc, bt = _paged_setup(kv_lens, nkv, hd)
@@ -403,7 +403,7 @@ def test_gemm_fp8_w8a8(m, n, k, splitk):
 @pytest.mark.parametrize("m,n,k,splitk,bn", [(1, 256, 256, 1, 0), (33, 256, 512, 1, 0), (128, 256, 384, 1, 0),
                                               (200, 384, 1024, 2, 0), (300, 256, 512, 1, 256)])
 def test_gemm_mxfp8_block_scaled(m, n, k, splitk, bn):
-    """tcgen05 kind::mxf8f6f4.block_scale: e4m3 operands with one UE8M0 scale per 32 K elements (scales in TMEM)."""
+    """MX block-scaled fp8: e4m3 operands with one UE8M0 scale per 32 K elements (applied per 32-K partial product)."""
     w, x = bf(n, k, scale=0.05, seed=1), bf(m, k, scale=2.0, seed=2)
     # block magnitudes spread over 2^-6..2^5 so that a wrong scale-factor address shows up as a large error
     x = (x.float() * torch.exp2(torch.randint(-6, 6, (m, k // 32), device="cuda").float()).repeat_interleave(32, 1)).to(torch.bfloat16)
@@ -483,10 +483,10 @@ def test_gemm_fused_epilogues_chain():
           torch_ref.gelu_tanh(out.float() @ wd.float().t() + bias))
 
 
-# ---------------------------------------------------------------- K12: dense layer fwd / bwd on the tcgen05 GEMM
+# ---------------------------------------------------------------- K12: dense layer fwd / bwd on the wgmma GEMM
 def test_dense_layer_forward_backward_on_tensor_cores():
     """legacy split-learning layer tasks (node.py layer_forward_train / layer_backward): tile-aligned shapes run on
-    the tcgen05 GEMM (bf16 operands, fp32 accumulation) and agree with the fp32 formulas."""
+    the wgmma GEMM (bf16 operands, fp32 accumulation) and agree with the fp32 formulas."""
     from bee2bee_b200 import model as mlp
 
     torch.manual_seed(0)
@@ -510,7 +510,7 @@ def test_dense_layer_forward_backward_on_tensor_cores():
         close(gb, g.mul((zr > 0).float()).sum(0) if act == "relu" else gb, rtol=1e-3, atol=1e-3)
 
 
-# ------------------------------------------------- TMA-multicast cluster GEMM (correct on hardware; not faster, so opt-in)
+# ------------------------------------------------- TMA-multicast cluster GEMM (opt-in)
 @pytest.mark.parametrize("mc", [2, 4])
 @pytest.mark.parametrize("m", [512, 300])
 def test_gemm_multicast_cluster(mc, m):
@@ -522,17 +522,16 @@ def test_gemm_multicast_cluster(mc, m):
         close(ops.gemm(w, x, bn=bn, splitk=1, mc=mc, epi=ops.EPI_RESIDUAL, residual=res), ref + res.float(), rtol=2e-2, atol=2e-2)
 
 
-@pytest.mark.parametrize("p_tmem", ["1", "0"])
-def test_attention_p_in_tmem_and_smem_variants(p_tmem):
-    """P kept in tensor memory (TS-form tcgen05.mma, the default) and the shared-memory P variant: the numerics
-    script must report the same error levels for both."""
+def test_attention_tc_numerics_script():
+    """The tensor-core attention numerics script (tools/attn_tc_check.py: prefill shapes against an fp32 reference)
+    runs end to end and reports small errors for every case."""
     import re
     import subprocess
     import sys
 
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     out = subprocess.run([sys.executable, os.path.join(root, "tools", "attn_tc_check.py")], capture_output=True, text=True,
-                         timeout=600, env=dict(os.environ, B2B_ATTN_P_TMEM=p_tmem))
+                         timeout=600)
     assert out.returncode == 0, out.stderr[-2000:]
     errs = [float(x) for x in re.findall(r"max_err ([0-9.]+)", out.stdout)]
     assert len(errs) >= 5 and max(errs) < 0.03, out.stdout

@@ -77,7 +77,7 @@ def test_engine_gpu_continuous_batching():
     assert [len(o) for o in outs] == [12] * 6
     assert all(0 <= t < eng.cfg.vocab_size for o in outs for t in o)
     # determinism: same seeds -> same tokens, independent of the decode burst length.  (The prompt set is kept
-    # identical: a 70-token prompt in the prefill chunk selects the tcgen05 attention kernel for the whole chunk,
+    # identical: a 70-token prompt in the prefill chunk selects the tensor-core attention kernel for the whole chunk,
     # whose bf16 rounding differs from the CUDA-core kernel used for short chunks.)
     eng2 = Engine("tiny-llama", device="cuda", max_batch=4, max_seq_len=256, decode_burst=3)
     outs2 = eng2.generate(prompts, sp)

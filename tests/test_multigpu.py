@@ -1,4 +1,4 @@
-"""Pieces over several B200s: the fused tail-GEMM -> NVLink peer store -> flag -> head-GEMM
+"""Pieces over several GPUs: the fused tail-GEMM -> NVLink peer store -> flag -> head-GEMM
 handoff, wavefront micro-batch groups and the token return path must reproduce the
 single-GPU result bit-for-bit (same kernels, same split-K, only the transport differs)."""
 import json

@@ -1,4 +1,4 @@
-"""First-light check + timing of the tcgen05 prefill attention against an fp32 reference."""
+"""First-light check + timing of the tensor-core prefill attention against an fp32 reference."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))

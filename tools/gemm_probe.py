@@ -1,4 +1,4 @@
-"""Quick numerical probe of the tcgen05 GEMM across tile/split configurations (prints, never asserts)."""
+"""Quick numerical probe of the wgmma GEMM across tile/split configurations (prints, never asserts)."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

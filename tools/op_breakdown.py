@@ -69,8 +69,8 @@ for B in (1, 32):
         us = e0.elapsed_time(e1) * 1e3 / (5 * 4 * NL)
         if kind != "layer":
             tot += us
-            ideal = wbytes[kind] / 6.477e6
-            print(f"B={B:2d} {kind:5s}: {us:6.1f} us   (weights at measured HBM bw: {ideal:5.1f} us, overhead {us - ideal:5.1f})", flush=True)
+            ideal = wbytes[kind] / 3.35e6       # H100 SXM data-sheet HBM3 bandwidth
+            print(f"B={B:2d} {kind:5s}: {us:6.1f} us   (weights at data-sheet HBM bw: {ideal:5.1f} us, overhead {us - ideal:5.1f})", flush=True)
         else:
-            print(f"B={B:2d} layer: {us:6.1f} us   (sum of isolated ops {tot:6.1f}; HBM floor {sum(wbytes.values()) / 6.477e6:5.1f})", flush=True)
+            print(f"B={B:2d} layer: {us:6.1f} us   (sum of isolated ops {tot:6.1f}; HBM floor {sum(wbytes.values()) / 3.35e6:5.1f})", flush=True)
     del piece

@@ -52,5 +52,5 @@ for B in [int(b) for b in os.environ.get("B", "32").split(",")]:
                     g.replay()
                 e1.record(s); s.synchronize()
             us = e0.elapsed_time(e1) * 1e3 / (5 * 4 * NL)
-            print(f"B={B} stages={stages} pf(upfront)={pf:3d}: {us:7.1f} us/layer  ({wb / us / 1e3:6.0f} GB/s, floor {wb / 6.477e6:5.1f} us)", flush=True)
+            print(f"B={B} stages={stages} pf(upfront)={pf:3d}: {us:7.1f} us/layer  ({wb / us / 1e3:6.0f} GB/s, data-sheet floor {wb / 3.35e6:5.1f} us)", flush=True)
     del piece
