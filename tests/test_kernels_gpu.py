@@ -115,9 +115,15 @@ def test_gemm_fused_rmsnorm(inline):
     close(out, ref, rtol=3e-2, atol=3e-2)
 
 
-@pytest.mark.parametrize("hd,nq,nkv", [(128, 4, 2), (256, 2, 1), (64, 4, 4)])
-def test_gemm_qkv_rope_append(hd, nq, nkv):
-    h, m, theta = 256, 6, 10000.0
+@pytest.mark.parametrize("hd,nq,nkv,quant", [
+    pytest.param(hd, nq, nkv, quant, id=f"{hd}-{nq}-{nkv}" + ("" if quant == "bf16" else f"-{quant}"))
+    for quant in ("bf16", "fp8", "mxfp8") for hd, nq, nkv in [(128, 4, 2), (256, 2, 1), (64, 4, 4)]])
+def test_gemm_qkv_rope_append(hd, nq, nkv, quant):
+    """QKV projection + RoPE + paged-KV append in the GEMM epilogue.  fp8 / mxfp8: the inputs are quantised the way
+    NativePiece._quant(..., with_rms=True) does (fp8: 1/rms folded into the per-token scale -> rstd; mxfp8: raw values +
+    the row's sum of squares -> sumsq), gamma is folded into the weights, and the reference is
+    rope(rms_norm(dequant(x)) @ dequant(W).T) on the quantised operands: only bf16 output rounding separates the two."""
+    h, m, theta, eps = 256, 6, 10000.0, 1e-5
     wq, wk, wv = bf(nq * hd, h, scale=0.05, seed=1), bf(nkv * hd, h, scale=0.05, seed=2), bf(nkv * hd, h, scale=0.05, seed=3)
     x = bf(m, h)
     w = torch.cat([ops.rope_interleave_rows(wq, nq, hd), ops.rope_interleave_rows(wk, nkv, hd), wv], 0).contiguous()
@@ -128,22 +134,51 @@ def test_gemm_qkv_rope_append(hd, nq, nkv):
     pos = torch.tensor([0, 1, 2, 70, 71, 500], device="cuda", dtype=torch.int32)
     slots = torch.tensor([5, 6, 64, 130, -1, 200], device="cuda", dtype=torch.int32)
     scale = 0.25
-    ops.gemm(w, x, epi=ops.EPI_QKV_ROPE, q_out=q_out, k_cache=kc, v_cache=vc, positions=pos, slots=slots,
-             n_q_heads=nq, n_kv_heads=nkv, head_dim=hd, rope_theta=theta, q_scale=scale)
-    torch.cuda.synchronize()
-    xf = x.float()
-    q = torch_ref.rope((xf @ wq.float().t()).view(1, m, nq, hd), pos.long()[None], theta)[0] * scale
-    k = torch_ref.rope((xf @ wk.float().t()).view(1, m, nkv, hd), pos.long()[None], theta)[0]
-    v = (xf @ wv.float().t()).view(m, nkv, hd)
+    kw = dict(epi=ops.EPI_QKV_ROPE, q_out=q_out, k_cache=kc, v_cache=vc, positions=pos, slots=slots,
+              n_q_heads=nq, n_kv_heads=nkv, head_dim=hd, rope_theta=theta, q_scale=scale)
     half = hd // 2
     perm = torch.arange(hd, device="cuda").view(2, half).t().reshape(-1)     # kernel layout: interleaved pairs
-    close(q_out.view(m, nq, hd), q[:, :, perm])
+    qd = nq * hd
+    if quant == "bf16":
+        ops.gemm(w, x, **kw)
+        xf = x.float()
+        wq_ref, wk_ref, wv_ref = wq.float(), wk.float(), wv.float()
+        tol = dict()
+    else:
+        gamma = (1 + 0.2 * torch.randn(h, device="cuda", generator=torch.Generator(device="cuda").manual_seed(7))).to(torch.bfloat16)
+        wf = ops.fold_gamma(w, gamma)
+        if quant == "fp8":
+            wq8, ws = ops.quantize_weight_fp8(wf)
+            xq, xs = ops.quant_fp8_rows(x, eps, with_rms=True)
+            ops.gemm(wq8, xq, rstd=xs, w_scale=ws, eps=eps, **kw)
+            wd = wq8.float() * ws[:, None]
+            xf = xq.float() * xs[:, None]                      # the per-token scale already holds 1/rms
+            rs_ref = torch.rsqrt(x.double().pow(2).mean(-1) + eps)
+            torch.testing.assert_close(xs.double(), x.double().abs().amax(-1) / 448 * rs_ref, rtol=1e-5, atol=0)
+        else:
+            wq8, sfa = ops.quantize_weight_mxfp8(wf)
+            ss = torch.empty(m, device="cuda")
+            xq, sfb = ops.quant_mxfp8_rows(x, 0, eps, sumsq_out=ss)
+            ops.gemm(wq8, xq, sfa=sfa, sfb=sfb, sumsq=ss, eps=eps, **kw)
+            wd = ops.mx_dequant(wq8, ops.mx_unchunk(sfa, wq8.shape[0], h, 128))
+            xf = ops.mx_dequant(xq, ops.mx_unchunk(sfb, m, h, ops.pick_bn_mx(m))) * torch.rsqrt(ss / h + eps)[:, None]
+        # the dequantised weight is in the kernel's interleaved row layout: back to the checkpoint layout for the reference
+        inv = torch.argsort(perm)
+        wq_ref = wd[:qd].view(nq, hd, h)[:, inv].reshape(qd, h)
+        wk_ref = wd[qd:qd + nkv * hd].view(nkv, hd, h)[:, inv].reshape(nkv * hd, h)
+        wv_ref = wd[qd + nkv * hd:]
+        tol = dict(rtol=6e-3, atol=0.0)                       # bf16 output rounding on the quantised operands
+    torch.cuda.synchronize()
+    q = torch_ref.rope((xf @ wq_ref.t()).view(1, m, nq, hd), pos.long()[None], theta)[0] * scale
+    k = torch_ref.rope((xf @ wk_ref.t()).view(1, m, nkv, hd), pos.long()[None], theta)[0]
+    v = (xf @ wv_ref.t()).view(m, nkv, hd)
+    close(q_out.view(m, nq, hd), q[:, :, perm], **tol)
     kflat, vflat = kc.view(-1, nkv, hd), vc.view(-1, nkv, hd)
     for i, s in enumerate(slots.tolist()):
         if s < 0:
             continue
-        close(kflat[s], k[i][:, perm])
-        close(vflat[s], v[i])
+        close(kflat[s], k[i][:, perm], **tol)
+        close(vflat[s], v[i], **tol)
     assert kflat[131].abs().sum() == 0   # the slot of the masked token stays untouched
 
 

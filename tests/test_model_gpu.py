@@ -34,6 +34,7 @@ def test_piece_matches_oracle(name, graphs):
     seqs = [SeqInit(slot=i, prompt=[t % V for t in p], pages=list(range(1 + 8 * i, 9 + 8 * i)), temperature=0.0,
                     top_p=1.0, repetition_penalty=1.0, seed=i) for i, p in enumerate(prompts)]
     runner.prefill(seqs)
+    runner.sync()          # prefill only enqueues on the runner's stream: read the first tokens after it
     caches = [oracle.new_cache() for _ in seqs]
     with torch.no_grad():
         ref_last = []
@@ -101,6 +102,7 @@ def test_piece_fp8_close_to_oracle(name, quant):
     seqs = [SeqInit(slot=i, prompt=[t % V for t in p], pages=[1 + 4 * i, 2 + 4 * i], temperature=0.0, top_p=1.0,
                     repetition_penalty=1.0, seed=i) for i, p in enumerate(prompts)]
     runner.prefill(seqs)
+    runner.sync()          # prefill only enqueues on the runner's stream: read the first tokens after it
     caches = [oracle.new_cache() for _ in seqs]
     with torch.no_grad():
         for s, c in zip(seqs, caches):
