@@ -243,7 +243,8 @@ __global__ void attn_merge_kernel(const AttnParams p, const int G) {
   pdl_wait();
   const int seq = blockIdx.x, kvh = blockIdx.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp >= G) return;
+  // an inactive sequence (q_len 0) has no partials (its split CTAs return at once) and no output row of its own
+  if (warp >= G || p.q_len[seq] <= 0) return;
   const int r = warp;                       // decode: QB = 1 -> row == head in group
   constexpr int DL = D / 32;
   float m = -INFINITY;
@@ -303,11 +304,12 @@ int attention_init() {
   return 0;
 }
 
-int launch_attention_merge(void* out, const int* q_start, const float* ws, int seqs, int n_q, int n_kv, int head_dim,
-                           int splits, cudaStream_t s) {
+int launch_attention_merge(void* out, const int* q_start, const int* q_len, const float* ws, int seqs, int n_q, int n_kv,
+                           int head_dim, int splits, cudaStream_t s) {
   AttnParams p{};
   p.out = static_cast<__nv_bfloat16*>(out);
   p.q_start = q_start;
+  p.q_len = q_len;
   p.ws = const_cast<float*>(ws);
   p.n_q = n_q; p.n_kv = n_kv; p.splits = splits;
   const int G = n_q / n_kv, R = attn_rows(G, 1);

@@ -409,7 +409,7 @@ int launch_attention_tc(const void* q, const void* k_cache, const void* v_cache,
     default: return -3;
   }
   if (rc == 0 && p.splits > 1)
-    rc = launch_attention_merge(out, q_start, ws, seqs, n_q, n_kv, head_dim, p.splits, s);
+    rc = launch_attention_merge(out, q_start, q_len, ws, seqs, n_q, n_kv, head_dim, p.splits, s);
   return rc;
 }
 

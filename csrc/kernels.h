@@ -40,8 +40,8 @@ int launch_attention_tc(const void* q, const void* k_cache, const void* v_cache,
                         int n_tokens, int n_pages, int n_q, int n_kv, int head_dim, int window, float softcap,
                         int splits, float* ws, void* q_out8, void* q_sf, int q_bn, cudaStream_t s);
 // merge pass of split-KV decode (shared by the CUDA-core and the tensor-core kernels)
-int launch_attention_merge(void* out, const int* q_start, const float* ws, int seqs, int n_q, int n_kv, int head_dim,
-                           int splits, cudaStream_t s);
+int launch_attention_merge(void* out, const int* q_start, const int* q_len, const float* ws, int seqs, int n_q, int n_kv,
+                           int head_dim, int splits, cudaStream_t s);
 int attention_init();
 
 // sampler.cu
