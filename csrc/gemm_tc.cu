@@ -13,7 +13,7 @@
 // memory), warp 8 = TMA producer; warps 0..3 then run the fused epilogue, one weight row per thread.
 //
 // Fused epilogues: residual add, SwiGLU/GeGLU, bias+GELU, RMSNorm scale of the *input* (gamma folded into W;
-// per-token 1/rms computed by the consumer warps while the producer fills the ring), RoPE + paged-KV append for
+// per-token 1/rms computed by the consumer warps inside the main loop, under the weight stream), RoPE + paged-KV append for
 // the QKV projection, and the NVLink piece handoff: the tail GEMM of piece i stores its tiles straight into
 // piece i+1's input buffer on the peer GPU and publishes a release flag; the head GEMM of piece i+1 prefetches
 // its weight tiles, acquires the flag, then TMA-loads the freshly written activations.
@@ -230,50 +230,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         }
       }
       if (p.norm_src != nullptr) {
+        // the statistics themselves are gathered inside the main loop (below)
         if (p.wait_flag != nullptr) {
           const uint32_t target = *reinterpret_cast<const volatile uint32_t*>(p.wait_epoch) + 1;
           wait_flag_ge(p.wait_flag, target);
-        }
-        // one warp per token, FOUR tokens x FOUR row segments in flight per lane (the loop is L2-latency
-        // bound: 16 independent 128-bit loads are issued before the first use)
-        constexpr int NW = GEMM_CONSUMERS / 32;
-        const int kv8 = p.k / 8;
-        for (int tr = warp; tr < ncol; tr += 4 * NW) {
-          float ss[4] = {0.f, 0.f, 0.f, 0.f};
-          const uint4* rowp[4];
-          bool live[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int tok = tok0 + col0 + tr + NW * u;
-            live[u] = (tr + NW * u < ncol) && tok < p.m_tok;
-            rowp[u] = reinterpret_cast<const uint4*>(p.norm_src + static_cast<size_t>(live[u] ? tok : tok0) * p.k);
-          }
-          for (int i0 = lane; i0 < kv8; i0 += 128) {
-            uint4 v[4][4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-#pragma unroll
-              for (int u = 0; u < 4; ++u)
-                v[j][u] = (live[u] && i0 + 32 * j < kv8) ? rowp[u][i0 + 32 * j] : make_uint4(0, 0, 0, 0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-#pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v[j][u]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  float2 f = __bfloat1622float2(h[e]);
-                  ss[u] += f.x * f.x + f.y * f.y;
-                }
-              }
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) ss[u] += __shfl_xor_sync(0xffffffffu, ss[u], o);
-            if (lane == 0 && tr + NW * u < ncol)
-              rstd_s[col0 + tr + NW * u] = live[u] ? rsqrtf(ss[u] / static_cast<float>(p.k) + p.eps) : 0.f;
-          }
         }
       } else {
         if constexpr (MX) {
@@ -316,9 +276,51 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         }
       }
     };
+    // Fused RMSNorm statistics, gathered under the weight stream: the ring is full when the consumers get here, and
+    // computing 1/rms up front would stall every CTA of the (one-wave) grid at once while HBM idles.  The result is
+    // only needed by the epilogue, so each k-block issues one step -- four 16-byte loads of one token row, sent before
+    // the stage wait and summed after its MMAs -- and the steps left over when the loop ends run after it.
+    // Warp w owns the slice columns w, w + 8, ...; a column takes ceil(k / 1024) steps.  Every token's sum runs in the
+    // same order as a plain per-warp loop (lane, 1024-element round, 256-element segment, pair, xor tree), so 1/rms
+    // does not depend on the schedule.  fp8 inputs bring their 1/rms in `rstd` / `sumsq` (the launcher refuses
+    // norm_from_x for them), so their instantiations carry none of this.
+    const int st_kv8 = p.k / 8;
+    const int st_rounds = (st_kv8 + 127) / 128;
+    const int st_ncol = (p.norm_src == nullptr) ? 0 : max(0, min(ncol, p.m_tok - tok0 - col0));   // live columns
+    int st_c = warp, st_r = 0;
+    float st_ss = 0.f;
+    auto stats_load = [&](uint4 (&v)[4]) {
+      const uint4* row = reinterpret_cast<const uint4*>(p.norm_src + static_cast<size_t>(tok0 + col0 + st_c) * p.k);
+      const int i0 = lane + 128 * st_r;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[j] = (i0 + 32 * j < st_kv8) ? row[i0 + 32 * j] : make_uint4(0, 0, 0, 0);
+    };
+    auto stats_add = [&](const uint4 (&v)[4]) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v[j]);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float2 f = __bfloat1622float2(h[e]);
+          st_ss += f.x * f.x + f.y * f.y;
+        }
+      }
+      if (++st_r == st_rounds) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) st_ss += __shfl_xor_sync(0xffffffffu, st_ss, o);
+        if (lane == 0) rstd_s[col0 + st_c] = rsqrtf(st_ss / static_cast<float>(p.k) + p.eps);
+        st_ss = 0.f;
+        st_r = 0;
+        st_c += GEMM_CONSUMERS / 32;
+      }
+    };
+
     int s = 0, prev = -1;
     uint32_t ph = 0;
     for (int kb = 0; kb < nkb; ++kb) {
+      const bool st_step = !FP8 && st_c < st_ncol;     // warp-uniform
+      uint4 st_v[4];
+      if (st_step) stats_load(st_v);
       mbar_wait(&full_bar[s], ph);
       if (threadIdx.x == 0 && kb == 0) B2B_DBG(3);
       const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(smem + s * STAGE_BYTES + wg * 64 * ROW_BYTES));
@@ -374,12 +376,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         if (prev >= 0) release(prev);
         prev = s;
       }
+      if (st_step) stats_add(st_v);
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
     if constexpr (!MX) {
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (prev >= 0) release(prev);
+    }
+    while (!FP8 && st_c < st_ncol) {
+      uint4 st_v[4];
+      stats_load(st_v);
+      stats_add(st_v);
     }
     if (threadIdx.x == 0) B2B_DBG(4);
 
