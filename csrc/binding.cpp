@@ -46,7 +46,7 @@ void gemm(const Tensor& w, const Tensor& x, int64_t out_ptr, int64_t ld_out, int
           // handoff
           int64_t wait_flag, int64_t wait_epoch, int64_t signal_flag, int64_t signal_epoch, int64_t done_counter,
           int64_t free_flag, int64_t bump_epoch, int64_t ack_flag, int64_t dbg, const OptT& w_scale,
-          const OptT& sfa, const OptT& sfb, int64_t mc, int64_t pf_tiles, int64_t stages, int64_t free_lag, int64_t out2_ptr,
+          const OptT& sfa, const OptT& sfb, int64_t stages, int64_t free_lag, int64_t out2_ptr,
           // fused MX quantisation of the output / RMSNorm statistics (raw addresses, 0 = off)
           int64_t q_out8, int64_t q_sf, int64_t ld_q, int64_t q_bn, int64_t sumsq_out, int64_t zero_buf, int64_t sumsq) {
   const bool fp8 = w.scalar_type() == at::kFloat8_e4m3fn;
@@ -81,7 +81,6 @@ void gemm(const Tensor& w, const Tensor& x, int64_t out_ptr, int64_t ld_out, int
   p.act_gelu = act_gelu ? 1 : 0;
   p.fp8 = fp8 ? 1 : 0;
   p.stages = static_cast<int8_t>(stages);
-  p.mc = static_cast<int8_t>(mc);      // experimental TMA-multicast cluster (0/1 = off)
   p.w_scale = ptr_or_null<const float>(w_scale);
   p.sfa = fp8 ? ptr_or_null<const uint8_t>(sfa) : nullptr;
   p.sfb = fp8 ? ptr_or_null<const uint8_t>(sfb) : nullptr;
@@ -260,13 +259,21 @@ void flag_signal(int64_t flag, int64_t epoch, int64_t bump_epoch, int64_t ack_fl
 }
 
 // -------------------------------------------------------------------- attention
-// query-chunk length from which the tensor-core prefill kernel is used (0 = never); env B2B_ATTN_TC_MIN_Q
-static int64_t g_attn_tc_min_q = [] {
-  const char* e = std::getenv("B2B_ATTN_TC_MIN_Q");
-  return e ? static_cast<int64_t>(std::atoi(e)) : static_cast<int64_t>(2);
-}();
+// query-chunk length from which prefill chunks run on the tensor-core kernel (0 = never, decode included)
+static int64_t g_attn_tc_min_q = 2;
 void set_attn_tc_min_q(int64_t v) { g_attn_tc_min_q = v; }
 int64_t get_attn_tc_min_q() { return g_attn_tc_min_q; }
+
+// The attention kernel of a call.  use_tc: -1 = default: decode (max_q == 1, the GQA group stacked into the MMA rows)
+// and prefill chunks of at least tc_min_q queries run on the tensor-core kernel; 1 = force the tensor-core kernel; 0 =
+// force the CUDA-core kernel.  The tensor-core kernel also needs tc_min_q > 0 and a GQA layout it supports; every other
+// call runs on the CUDA-core kernel.
+bool attention_uses_tc(int64_t max_q, int64_t n_q, int64_t n_kv, int64_t head_dim, int64_t use_tc) {
+  if (use_tc == 0 || g_attn_tc_min_q <= 0 ||
+      !b2b::attention_tc_supported(static_cast<int>(n_q), static_cast<int>(n_kv), static_cast<int>(head_dim)))
+    return false;
+  return use_tc > 0 || max_q == 1 || max_q >= g_attn_tc_min_q;
+}
 
 void attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& out,
                const Tensor& block_table, const Tensor& q_start, const Tensor& q_len, const Tensor& kv_len,
@@ -276,17 +283,14 @@ void attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, co
   c10::cuda::CUDAGuard guard(q.device());
   TORCH_CHECK(block_table.scalar_type() == at::kInt && q_len.scalar_type() == at::kInt, "int32 metadata expected");
   const int seqs = static_cast<int>(q_len.size(0));
-  // use_tc: -1 = by query-chunk length (prefill chunks), 1 = force the tensor-core kernel (decode: one-token query blocks,
-  // the GQA group stacked into the MMA rows), 0 = force the CUDA-core kernel (split-KV decode of few sequences)
-  const bool want_tc = use_tc < 0 ? (max_q >= g_attn_tc_min_q && g_attn_tc_min_q > 0) : (use_tc > 0 && g_attn_tc_min_q > 0);
-  if (want_tc && splits > 1 && max_q == 1) {
+  const bool tc = attention_uses_tc(max_q, n_q, n_kv, head_dim, use_tc);
+  // split-KV: the CUDA-core kernel, or the tensor-core kernel on decode (it runs prefill chunks unsplit)
+  if (splits > 1 && (!tc || max_q == 1)) {
     TORCH_CHECK(ws.has_value(), "split-KV needs a workspace");
     const int64_t R = b2b::attn_rows(static_cast<int>(n_q / n_kv), 1);
     TORCH_CHECK(ws->numel() >= seqs * n_kv * splits * R * (head_dim + 2), "attention workspace too small");
   }
-  if (want_tc &&
-      b2b::attention_tc_supported(static_cast<int>(n_q), static_cast<int>(n_kv), static_cast<int>(head_dim))) {
-    // prefill chunk: tensor-core flash attention
+  if (tc) {
     check(b2b::launch_attention_tc(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(),
                                    reinterpret_cast<const int*>(block_table.data_ptr()),
                                    reinterpret_cast<const int*>(q_start.data_ptr()),
@@ -301,11 +305,6 @@ void attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, co
     return;
   }
   TORCH_CHECK(fq_out == 0, "fused output quantisation needs the tensor-core attention kernel");
-  if (splits > 1) {
-    TORCH_CHECK(ws.has_value(), "split-KV needs a workspace");
-    const int64_t R = b2b::attn_rows(static_cast<int>(n_q / n_kv), 1);
-    TORCH_CHECK(ws->numel() >= seqs * n_kv * splits * R * (head_dim + 2), "attention workspace too small");
-  }
   check(b2b::launch_attention(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), out.data_ptr(),
                               reinterpret_cast<const int*>(block_table.data_ptr()),
                               reinterpret_cast<const int*>(q_start.data_ptr()),
@@ -433,6 +432,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flag_signal", &flag_signal);
   m.def("decode_advance", &decode_advance);
   m.def("attention", &attention);
+  m.def("attention_uses_tc", &attention_uses_tc, py::arg("max_q"), py::arg("n_q"), py::arg("n_kv"), py::arg("head_dim"),
+        py::arg("use_tc") = -1);
   m.def("set_attn_tc_min_q", &set_attn_tc_min_q);
   m.def("get_attn_tc_min_q", &get_attn_tc_min_q);
   m.def("sample", &sample);

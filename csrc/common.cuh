@@ -91,24 +91,6 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorM
       "r"(c1), "l"(policy)
       : "memory");
 }
-// Multicast variant: the box lands at the same shared-memory offset in every CTA of `cta_mask` and completes
-// bytes on the mbarrier at the same offset in each of them.
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0,
-                                                      int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-      "h"(cta_mask)
-      : "memory");
-}
-// L2-only prefetch of a tile (no shared-memory destination, no mbarrier): keeps HBM busy with the weight tiles a CTA
-// will need beyond its shared-memory ring while the kernel still waits on its producer (PDL / peer flag).
-__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1)
-               : "memory");
-}
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -181,11 +163,6 @@ __device__ __forceinline__ uint2 ld_dsmem_v2u32(uint32_t cluster_addr) {
   uint2 v;
   asm volatile("ld.shared::cluster.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(cluster_addr) : "memory");
   return v;
-}
-// arrive on the mbarrier at this shared-memory offset in CTA `cta_rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta_rank) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(mapa_smem(smem_u32(bar), cta_rank))
-               : "memory");
 }
 __device__ __forceinline__ void st_dsmem_v2(uint32_t cluster_addr, float a, float b) {
   asm volatile("st.shared::cluster.v2.f32 [%0], {%1,%2};" ::"r"(cluster_addr), "f"(a), "f"(b) : "memory");

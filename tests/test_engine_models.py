@@ -314,6 +314,30 @@ def test_split_k_heuristic_matches_the_measured_optimum():
     assert ops.pick_prefill_tile(256, 512, 256) == (128, 3, 1)             # tiny models: too few k-blocks to split
 
 
+def test_attention_kernel_choice():
+    """the extension's one attention-kernel decision (host code, no launch): decode and prefill chunks of >= tc_min_q
+    queries run on the tensor-core kernel when it supports the GQA layout; the fused e4m3 output needs that kernel
+    without split-KV"""
+    from bee2bee_b200 import ops
+
+    uses = lambda max_q, use_tc=-1, g=4, d=128: ops.native().attention_uses_tc(max_q, 2 * g, 2, d, use_tc)  # noqa: E731
+    old = ops.get_attn_tc_min_q()
+    try:
+        ops.set_attn_tc_min_q(16)
+        assert [uses(q) for q in (0, 1, 2, 15, 16, 500)] == [False, True, False, False, True, True]
+        assert all(uses(q, 1) for q in (0, 1, 2, 15)) and not any(uses(q, 0) for q in (1, 16))
+        assert not any(uses(q, u, g=g) for q in (1, 16) for u in (-1, 1) for g in (3, 12, 32))
+        assert not any(uses(q, u, d=96) for q in (1, 16) for u in (-1, 1))
+        assert ops.attention_fuses_quant(1, 8, 2, 128, 1) and not ops.attention_fuses_quant(1, 8, 2, 128, 4)
+        assert ops.attention_fuses_quant(16, 8, 2, 128, 4) and not ops.attention_fuses_quant(15, 8, 2, 128, 1)
+        assert not ops.attention_fuses_quant(1, 24, 2, 128, 1)
+        ops.set_attn_tc_min_q(0)
+        assert not any(uses(q, u) for q in (1, 16) for u in (-1, 1))
+        assert not ops.attention_fuses_quant(1, 8, 2, 128, 1)
+    finally:
+        ops.set_attn_tc_min_q(old)
+
+
 def test_weights_policy_random_init_is_opt_in(monkeypatch, tmp_path):
     """ADVICE r1: `serve-hf --model llama-3-8b` must not silently serve noise"""
     from bee2bee_b200.models.weights import WEIGHT_SOURCE, WeightsUnavailable, load_or_init

@@ -52,12 +52,13 @@ def test_gemm_splitk_cluster(splitk, m):
     close(ops.gemm(w, x, splitk=splitk), x.float() @ w.float().t())       # cluster / DSMEM kernel
 
 
-@pytest.mark.parametrize("bn,splitk,stages", [(256, 2, 0), (256, 4, 0), (128, 2, 3), (128, 4, 3), (128, 2, 0)])
+@pytest.mark.parametrize("bn,splitk,stages", [(256, 2, 0), (256, 4, 0), (128, 2, 3), (128, 4, 3), (128, 2, 0),
+                                               (128, 1, 0), (256, 1, 0)])
 @pytest.mark.parametrize("m", [256, 300, 512])
 def test_gemm_prefill_splitk_tiles(bn, splitk, stages, m):
     """the (token tile, split-K, ring depth) combinations ops.pick_prefill_tile emits for under-filled prefill GEMMs:
-    cluster split-K with the DSMEM reduce-scatter on 128 / 256-wide token tiles, plain and residual epilogues, ragged
-    last token tile"""
+    cluster split-K with the DSMEM reduce-scatter on 128 / 256-wide token tiles, and the same tiles without split-K,
+    plain and residual epilogues, ragged last token tile"""
     w, x, r = bf(512, 4096, scale=0.03), bf(m, 4096), bf(m, 512)
     ref = x.float() @ w.float().t()
     close(ops.gemm(w, x, bn=bn, splitk=splitk, stages=stages), ref)
@@ -303,6 +304,37 @@ def test_attention_decode_split_kv(splits, use_tc, hd, nq, nkv):
     close(out, _attn_ref(q, kc, vc, bt, [1] * S, kv_lens, nq, nkv, hd, 0, 0.0))
 
 
+@pytest.mark.parametrize("splits", [1, 4])
+@pytest.mark.parametrize("hd,nq,nkv", [(128, 8, 2), (64, 16, 1)])
+def test_attention_decode_default_kernel(hd, nq, nkv, splits):
+    """decode with the default use_tc = -1 on a layout the tensor-core kernel supports: the bytes of use_tc = 1, and
+    with tc_min_q = 0 the bytes of use_tc = 0"""
+    kv_lens = [1, 65, 300, 1000]
+    S = len(kv_lens)
+    kc, vc, bt = _paged_setup(kv_lens, nkv, hd)
+    q = bf(S, nq * hd, scale=0.3)
+    ws = torch.zeros(S * nkv * splits * 16 * (hd + 2), device="cuda") if splits > 1 else None
+    ar = torch.arange(S, device="cuda", dtype=torch.int32)
+    ones = torch.ones(S, device="cuda", dtype=torch.int32)
+    kvl = torch.tensor(kv_lens, device="cuda", dtype=torch.int32)
+
+    def run(use_tc):
+        out = torch.zeros_like(q)
+        ops.attention(q, kc, vc, out, bt, ar, ones, kvl, max_q=1, n_q=nq, n_kv=nkv, head_dim=hd, splits=splits, ws=ws,
+                      use_tc=use_tc)
+        return out
+
+    tc, cc = run(1), run(0)
+    assert not torch.equal(tc, cc)          # the kernels round differently, so the bytes tell which one ran
+    assert torch.equal(run(-1), tc)
+    old = ops.get_attn_tc_min_q()
+    ops.set_attn_tc_min_q(0)
+    try:
+        assert torch.equal(run(-1), cc)
+    finally:
+        ops.set_attn_tc_min_q(old)
+
+
 @pytest.mark.parametrize("hd,nq,nkv", [(128, 8, 2), (64, 2, 2), (256, 2, 1)])
 @pytest.mark.parametrize("window", [0, 50])
 def test_attention_prefill(hd, nq, nkv, window):
@@ -544,17 +576,6 @@ def test_dense_layer_forward_backward_on_tensor_cores():
         close(gW, Wr.grad, rtol=3e-2, atol=1e-1)
         close(gb, g.mul((zr > 0).float()).sum(0) if act == "relu" else gb, rtol=1e-3, atol=1e-3)
 
-
-# ------------------------------------------------- TMA-multicast cluster GEMM (opt-in)
-@pytest.mark.parametrize("mc", [2, 4])
-@pytest.mark.parametrize("m", [512, 300])
-def test_gemm_multicast_cluster(mc, m):
-    n, k = 1024, 1024
-    w, x, res = bf(n, k, scale=0.05, seed=1), bf(m, k, seed=2), bf(m, n, seed=3)
-    ref = x.float() @ w.float().t()
-    for bn in (128, 256):
-        close(ops.gemm(w, x, bn=bn, splitk=1, mc=mc), ref, rtol=2e-2, atol=2e-2)
-        close(ops.gemm(w, x, bn=bn, splitk=1, mc=mc, epi=ops.EPI_RESIDUAL, residual=res), ref + res.float(), rtol=2e-2, atol=2e-2)
 
 
 def test_attention_tc_numerics_script():
