@@ -338,6 +338,14 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
         "sample");
 }
 
+// CTAs per sequence that `sample` runs a batch of `batch` rows at on the current device (0 = vocabulary too large)
+int64_t sample_cluster_size(int64_t batch, int64_t vocab) {
+  int dev = 0, sms = 0;
+  check(static_cast<int>(cudaGetDevice(&dev)), "cudaGetDevice");
+  check(static_cast<int>(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)), "cudaDeviceGetAttribute");
+  return b2b::sample_cluster_size(static_cast<int>(batch), static_cast<int>(vocab), sms);
+}
+
 void set_decode_state(const Tensor& positions, const Tensor& kv_len, const Tensor& q_len, int64_t row_map, int64_t kvlen,
                       int64_t n) {
   c10::cuda::CUDAGuard guard(positions.device());
@@ -437,6 +445,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("set_attn_tc_min_q", &set_attn_tc_min_q);
   m.def("get_attn_tc_min_q", &get_attn_tc_min_q);
   m.def("sample", &sample);
+  m.def("sample_cluster_size", &sample_cluster_size, py::arg("batch"), py::arg("vocab"));
   m.def("mark_seen", &mark_seen);
   m.def("set_decode_state", &set_decode_state);
   m.def("fetch_window", &fetch_window);

@@ -50,6 +50,9 @@ int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* pee
                   const float* temperature, const float* top_p, const float* rep_penalty, const uint32_t* seeds,
                   const uint32_t* step, uint32_t* signal_flag, uint32_t* signal_epoch, uint32_t* done_counter,
                   const int* row_map, cudaStream_t s);
+// CTAs per sequence (1, 2, 4 or 8) that launch_sample runs a batch at on a device with `sms` SMs; 0 = the vocabulary
+// does not fit in shared memory at any cluster size
+int sample_cluster_size(int batch, int vocab, int sms);
 int launch_set_decode_state(int* positions, int* kv_len, int* q_len, const int* row_map, const int* kvlen, int n,
                             cudaStream_t s);
 // token-window read-back: wait for up to `n_waits` (flag, target) pairs, then out[b, j] = history[b, (cursor[b] + j) % stride]

@@ -441,6 +441,15 @@ __global__ void mark_seen_kernel(const int* ids, const int* seq_of, uint32_t* se
   atomicOr(&seen[static_cast<size_t>(seq_of[i]) * words + (id >> 5)], 1u << (id & 31));
 }
 
+// cluster size: the slice must fit in shared memory; beyond that use more SMs while the grid is below one wave
+int sample_cluster_size(int batch, int vocab, int sms) {
+  int cs = 1;
+  while (cs < MAX_CS && (vocab + cs - 1) / cs > MAX_SLICE) cs *= 2;
+  if ((vocab + cs - 1) / cs > MAX_SLICE) return 0;
+  while (cs < MAX_CS && batch * cs * 2 <= sms) cs *= 2;
+  return cs;
+}
+
 int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* peer_tokens, int* history,
                   const int* hist_pos, int* hist_pos_out, int hist_stride, int batch, int vocab, int ld, float softcap,
                   const float* temperature, const float* top_p, const float* rep_penalty, const uint32_t* seeds,
@@ -451,10 +460,7 @@ int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* pee
   p.hist_pos = hist_pos; p.hist_pos_out = hist_pos_out; p.hist_stride = hist_stride; p.vocab = vocab; p.ld = ld; p.softcap = softcap;
   p.temperature = temperature; p.top_p = top_p; p.rep_penalty = rep_penalty; p.seeds = seeds; p.step = step;
   p.signal_flag = signal_flag; p.signal_epoch = signal_epoch; p.done_counter = done_counter; p.row_map = row_map;
-  // cluster size: the slice must fit in shared memory; beyond that use more SMs while the grid is below one wave
-  int cs = 1;
-  while (cs < MAX_CS && (vocab + cs - 1) / cs > MAX_SLICE) cs *= 2;
-  if ((vocab + cs - 1) / cs > MAX_SLICE) return -6;
+  if (sample_cluster_size(1, vocab, 0) == 0) return -6;
   static int sm_count[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -463,7 +469,7 @@ int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* pee
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -9;
     if (dev < 64) sm_count[dev] = sms;
   }
-  while (cs < MAX_CS && batch * cs * 2 <= sms) cs *= 2;
+  const int cs = sample_cluster_size(batch, vocab, sms);
   const int W = (((vocab + cs - 1) / cs) + 127) & ~127;
   const size_t smem = sizeof(SampShared) + static_cast<size_t>(W) * sizeof(float);
   static bool attr_set[64] = {};
