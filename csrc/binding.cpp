@@ -150,6 +150,16 @@ int64_t gemm_max_splitk(int64_t bn, int64_t epi, int64_t stages) {
   return b2b::gemm_tc_max_splitk(static_cast<int>(bn), static_cast<int>(epi), static_cast<int>(stages));
 }
 
+// (ring depth, cluster split-K) that `gemm` runs for these arguments; fp8: 0 = bf16, 1 = per-row fp8, 2 = MX fp8
+std::tuple<int64_t, int64_t> gemm_resolve(int64_t bn, int64_t epi, int64_t k, int64_t fp8, int64_t stages,
+                                          int64_t splitk) {
+  int st = 0, sk = 0;
+  check(b2b::gemm_tc_resolve(static_cast<int>(bn), static_cast<int>(epi), static_cast<int>(k), static_cast<int>(fp8),
+                             static_cast<int>(stages), static_cast<int>(splitk), &st, &sk),
+        "gemm_resolve");
+  return {st, sk};
+}
+
 void init_kernels(int64_t device) {
   c10::cuda::CUDAGuard guard(static_cast<c10::DeviceIndex>(device));
   check(b2b::gemm_tc_init(), "gemm_tc_init");
@@ -426,6 +436,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "bee2bee_b200 native sm_90a kernels + NVLink peer-memory runtime";
   m.def("gemm", &gemm);
   m.def("gemm_max_splitk", &gemm_max_splitk);
+  m.def("gemm_resolve", &gemm_resolve, py::arg("bn"), py::arg("epi"), py::arg("k"), py::arg("fp8"), py::arg("stages"),
+        py::arg("splitk"));
   m.def("init_kernels", &init_kernels);
   m.def("set_pdl", &set_pdl);
   m.def("get_pdl", &get_pdl);

@@ -778,22 +778,37 @@ int gemm_tc_max_splitk(int bn, int epi, int stages) {
   return best;
 }
 
+int gemm_tc_resolve(int bn, int epi, int k, int fp8, int stages, int splitk, int* stages_out, int* splitk_out) {
+  if (bn != 16 && bn != 32 && bn != 64 && bn != 128 && bn != 256) return -3;
+  if (fp8 == 2 && bn < 32) return -7;   // MX scale-factor chunks are laid out for token tiles of >= 32
+  const int dflt = gemm_tc_default_stages(bn);
+  if (stages <= 0 || stages > dflt) stages = dflt;
+  if (stages < 2) stages = 2;
+  if (splitk < 1) splitk = 1;
+  if (splitk > 8) splitk = 8;
+  const int smax = gemm_tc_max_splitk(bn, epi, stages);
+  if (splitk > smax) splitk = smax;
+  const int nkb = k / (fp8 ? ROW_BYTES : ROW_BYTES / 2);
+  if (splitk > nkb) splitk = nkb;
+  while (splitk & (splitk - 1)) --splitk;      // cluster reduce-scatter: power of two (divides the token tile)
+  *stages_out = stages;
+  *splitk_out = splitk;
+  return 0;
+}
+
 int launch_gemm_tc(const GemmParams& p_in, const void* w, const void* x, int bn, cudaStream_t stream) {
   GemmParams p = p_in;
   const int elt = p.fp8 ? 1 : 2;
   const int bke = ROW_BYTES / elt;
   if (p.n_out % BM != 0 || p.k % bke != 0 || p.m_tok <= 0) return -2;
-  if (p.splitk < 1) p.splitk = 1;
-  if (p.splitk > 8) p.splitk = 8;
   {
-    const int dflt = gemm_tc_default_stages(bn);
-    if (p.stages <= 0 || p.stages > dflt) p.stages = dflt;
-    if (p.stages < 2) p.stages = 2;
+    int stages = 0, splitk = 0;
+    const int qm = p.fp8 ? (p.sfa != nullptr ? 2 : 1) : 0;
+    const int r = gemm_tc_resolve(bn, p.epi, p.k, qm, p.stages, p.splitk, &stages, &splitk);
+    if (r) return r;
+    p.stages = static_cast<int8_t>(stages);
+    p.splitk = static_cast<int8_t>(splitk);
   }
-  const int smax = gemm_tc_max_splitk(bn, p.epi, p.stages);
-  if (p.splitk > smax) p.splitk = smax;
-  if (p.splitk > p.k / bke) p.splitk = p.k / bke;
-  while (p.splitk & (p.splitk - 1)) --p.splitk;      // cluster reduce-scatter: power of two (divides the token tile)
   CUtensorMap tw, tx;
   int r = make_tmap(&tw, w, p.n_out, p.k, p.k, BM, elt);
   if (r) return r;

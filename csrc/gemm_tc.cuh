@@ -91,6 +91,11 @@ struct GemmParams {
 
 // Host launcher (gemm_tc.cu). Returns cudaError_t as int.
 int gemm_tc_max_splitk(int bn, int epi, int stages);
+// The (ring depth, cluster split-K) a launch with these arguments runs: `stages` <= 0 or above the tile's default ->
+// the default, then at least 2; `splitk` clamped to 1..8, to gemm_tc_max_splitk, to the number of k-blocks, then
+// rounded down to a power of two.  fp8: 0 = bf16, 1 = per-row fp8, 2 = MX fp8.  Returns 0, -3 (unknown bn) or -7 (MX
+// at bn 16).
+int gemm_tc_resolve(int bn, int epi, int k, int fp8, int stages, int splitk, int* stages_out, int* splitk_out);
 int launch_gemm_tc(const GemmParams& p, const void* w, const void* x, int bn, cudaStream_t stream);
 
 }  // namespace b2b
