@@ -176,6 +176,10 @@ class Engine:
         self.device = torch.device(device)
         if self.device.type == "cuda" and self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
+        if self.cfg.rope_theta <= 0:
+            # learned absolute positions (GPT-2): a sequence may not outgrow the position table; submit() trims prompts
+            # and the generation budget to this length
+            max_seq_len = min(max_seq_len, self.cfg.max_position)
         self.max_batch, self.max_seq_len, self.decode_burst = max_batch, max_seq_len, max(1, decode_burst)
         self.rank, self.world, self.control_group = rank, world, control_group
         self.h2d_bytes = 0

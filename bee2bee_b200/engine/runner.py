@@ -82,6 +82,9 @@ class GpuRunner:
                  max_seq_len: int = 4096, max_prefill_tokens: int = 2048, num_pages: int = 0, seed: int = 0,
                  hist_len: int = 0, control_group=None, use_graphs: bool = True, quant: str = "bf16"):
         assert max_batch % groups == 0, "max_batch must be divisible by the number of micro-batch groups"
+        if cfg.rope_theta <= 0 and max_seq_len > cfg.max_position:
+            # learned absolute positions: the embed kernel reads pos_table[position], a table of max_position rows
+            raise ValueError(f"{cfg.name}: max_seq_len {max_seq_len} exceeds the {cfg.max_position} learned positions")
         self.cfg, self.rank, self.world = cfg, rank, world
         self.device = torch.device(device if device is not None else f"cuda:{rank}")
         torch.cuda.set_device(self.device)

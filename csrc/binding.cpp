@@ -167,12 +167,29 @@ void init_kernels(int64_t device) {
 }
 
 // ----------------------------------------------------------------- elementwise
+// The elementwise kernels index every operand by the row length of x: a bf16 operand of another size or dtype would be
+// read or written out of bounds, so each is checked here.
+void check_bf16_numel(const Tensor& t, int64_t numel, const char* name) {
+  check_bf16(t, name);
+  TORCH_CHECK(t.numel() == numel, name, " has ", t.numel(), " elements, expected ", numel);
+}
+
 void rmsnorm(const Tensor& x, const Tensor& gamma, const OptT& residual, const OptT& out, const OptT& rstd_out,
              double eps, bool gemma_plus_one) {
   check_bf16(x, "x");
+  TORCH_CHECK(x.dim() >= 1 && x.size(-1) > 0, "rmsnorm: x must have a nonempty last dimension");
   c10::cuda::CUDAGuard guard(x.device());
   const int h = static_cast<int>(x.size(-1));
   const int tokens = static_cast<int>(x.numel() / h);
+  if (out.has_value() && out->defined()) {
+    check_bf16_numel(gamma, h, "rmsnorm: gamma");
+    check_bf16_numel(*out, x.numel(), "rmsnorm: out");
+    if (residual.has_value() && residual->defined()) check_bf16_numel(*residual, x.numel(), "rmsnorm: residual");
+  }
+  if (rstd_out.has_value() && rstd_out->defined())
+    TORCH_CHECK(rstd_out->is_cuda() && rstd_out->scalar_type() == at::kFloat && rstd_out->is_contiguous() &&
+                    rstd_out->numel() >= tokens, "rmsnorm: rstd_out must be a contiguous CUDA fp32 tensor of >= ", tokens,
+                " elements");
   check(b2b::launch_rmsnorm(x.data_ptr(), gamma.data_ptr(), ptr_or_null<void>(residual), ptr_or_null<void>(out),
                             ptr_or_null<float>(rstd_out), tokens, h, static_cast<float>(eps), gemma_plus_one ? 1 : 0,
                             cur_stream()),
@@ -181,8 +198,12 @@ void rmsnorm(const Tensor& x, const Tensor& gamma, const OptT& residual, const O
 
 void layernorm(const Tensor& x, const Tensor& gamma, const Tensor& beta, const Tensor& out, double eps) {
   check_bf16(x, "x");
+  TORCH_CHECK(x.dim() >= 1 && x.size(-1) > 0, "layernorm: x must have a nonempty last dimension");
   c10::cuda::CUDAGuard guard(x.device());
   const int h = static_cast<int>(x.size(-1));
+  check_bf16_numel(gamma, h, "layernorm: gamma");
+  check_bf16_numel(beta, h, "layernorm: beta");
+  check_bf16_numel(out, x.numel(), "layernorm: out");
   check(b2b::launch_layernorm(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), out.data_ptr(),
                               static_cast<int>(x.numel() / h), h, static_cast<float>(eps), cur_stream()),
         "layernorm");
@@ -191,8 +212,21 @@ void layernorm(const Tensor& x, const Tensor& gamma, const Tensor& beta, const T
 void embed(int64_t ids_ptr, const Tensor& table, const OptT& pos_table, const OptT& positions, const Tensor& out,
            double scale, int64_t tok_flag, int64_t tok_epoch, int64_t pf_flag, int64_t pf_need) {
   check_bf16(table, "table");
+  TORCH_CHECK(table.dim() == 2 && table.size(0) > 0 && table.size(1) > 0, "embed: table must be [vocab, h]");
   c10::cuda::CUDAGuard guard(table.device());
   const int h = static_cast<int>(table.size(1));
+  check_bf16(out, "embed: out");
+  TORCH_CHECK(out.numel() % h == 0, "embed: out has ", out.numel(), " elements, not a multiple of h = ", h);
+  const bool has_pos = pos_table.has_value() && pos_table->defined();
+  TORCH_CHECK(has_pos == (positions.has_value() && positions->defined()), "embed: pos_table and positions go together");
+  if (has_pos) {
+    check_bf16(*pos_table, "embed: pos_table");
+    TORCH_CHECK(pos_table->dim() == 2 && pos_table->size(0) > 0 && pos_table->size(1) == h, "embed: pos_table must be [n_pos, ",
+                h, "]");
+    TORCH_CHECK(positions->is_cuda() && positions->scalar_type() == at::kInt && positions->is_contiguous() &&
+                    positions->numel() >= out.numel() / h,
+                "embed: positions must be contiguous CUDA int32 with one entry per token");
+  }
   check(b2b::launch_embed(as_ptr<const int>(ids_ptr), table.data_ptr(), ptr_or_null<void>(pos_table),
                           ptr_or_null<const int>(positions), out.data_ptr(), static_cast<int>(out.numel() / h), h,
                           static_cast<int>(table.size(0)), static_cast<float>(scale), as_ptr<const uint32_t>(tok_flag),
@@ -204,6 +238,16 @@ void embed(int64_t ids_ptr, const Tensor& table, const OptT& pos_table, const Op
 void kv_append(const Tensor& qkv, const Tensor& q_out, const Tensor& k_cache, const Tensor& v_cache,
                const Tensor& slots, int64_t q_dim, int64_t kv_dim, double q_scale) {
   check_bf16(qkv, "qkv");
+  TORCH_CHECK(q_dim > 0 && kv_dim > 0 && qkv.dim() == 2 && qkv.size(1) == q_dim + 2 * kv_dim,
+              "kv_append: qkv must be [T, q_dim + 2 * kv_dim] = [T, ", q_dim + 2 * kv_dim, "]");
+  check_bf16(q_out, "kv_append: q_out");
+  TORCH_CHECK(q_out.numel() >= qkv.size(0) * q_dim, "kv_append: q_out holds fewer than T rows of q_dim");
+  check_bf16(k_cache, "kv_append: k_cache");
+  check_bf16(v_cache, "kv_append: v_cache");
+  TORCH_CHECK(k_cache.numel() % kv_dim == 0 && v_cache.numel() == k_cache.numel(),
+              "kv_append: k_cache and v_cache must be equal-sized rows of kv_dim");
+  TORCH_CHECK(slots.is_cuda() && slots.scalar_type() == at::kInt && slots.is_contiguous() && slots.numel() >= qkv.size(0),
+              "kv_append: slots must be contiguous CUDA int32 with one entry per token");
   c10::cuda::CUDAGuard guard(qkv.device());
   check(b2b::launch_kv_append(qkv.data_ptr(), q_out.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                               reinterpret_cast<const int*>(slots.data_ptr()), static_cast<int>(qkv.size(0)),
@@ -214,6 +258,8 @@ void kv_append(const Tensor& qkv, const Tensor& q_out, const Tensor& k_cache, co
 
 void add(const Tensor& a, const Tensor& b, const Tensor& out) {
   check_bf16(a, "a");
+  check_bf16_numel(b, a.numel(), "add: b");
+  check_bf16_numel(out, a.numel(), "add: out");
   c10::cuda::CUDAGuard guard(a.device());
   check(b2b::launch_add(a.data_ptr(), b.data_ptr(), out.data_ptr(), static_cast<size_t>(a.numel()), cur_stream()),
         "add");

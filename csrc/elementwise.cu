@@ -6,6 +6,8 @@
 
 #include <cuda_fp8.h>
 
+#include <cfloat>
+
 #include "common.cuh"
 #include "launch.cuh"
 
@@ -177,7 +179,7 @@ __global__ void add_kernel(const __nv_bfloat16* __restrict__ a, const __nv_bfloa
   reinterpret_cast<uint4*>(out)[i] = o;
 }
 
-// Per-token dynamic fp8 (e4m3) quantisation of a GEMM input: q = x / s, s = amax / 448.
+// Per-token dynamic fp8 (e4m3) quantisation of a GEMM input: q = x / s, s = max(amax / 448, FLT_MIN).
 // scale_out[t] = s (x optional 1/rms of the row, so a following fp8 GEMM with gamma folded into
 // its weights performs the whole RMSNorm + projection).  One CTA per token.
 __global__ void quant_fp8_rows_kernel(const __nv_bfloat16* __restrict__ x, uint8_t* __restrict__ q,
@@ -214,7 +216,9 @@ __global__ void quant_fp8_rows_kernel(const __nv_bfloat16* __restrict__ x, uint8
   amax = sh[0];
   __syncthreads();
   ss = block_sum(ss, sh);
-  const float s = amax > 0.f ? amax / 448.f : 1.f;
+  // FLT_MIN floor: under --use_fast_math a subnormal amax / 448 (amax < 448 FLT_MIN) flushes to 0, and 1 / 0 = inf
+  // would turn the row into +-448 and NaN bytes; with s = FLT_MIN every |x / s| stays below 448
+  const float s = amax > 0.f ? fmaxf(amax / 448.f, FLT_MIN) : 1.f;
   const float inv = 1.f / s;
   if (threadIdx.x == 0) scale_out[t] = with_rms ? s * rsqrtf(ss / h + eps) : s;
   uint2* qrow = reinterpret_cast<uint2*>(q + static_cast<size_t>(t) * h);

@@ -176,6 +176,21 @@ def test_engine_eos_stop_and_streaming_thread():
     assert got == first and req.finish_reason == "length" and req.ttft_ms > 0
 
 
+def test_learned_positions_bound_the_sequence_length():
+    """GPT-2 has a table of max_position learned positions: the engine clamps its context to it (prompts and the
+    generation budget are trimmed to fit), and the GPU runner refuses a longer one before it touches a device"""
+    from bee2bee_b200.engine.runner import GpuRunner
+    cfg = resolve_config("tiny-gpt2")
+    assert cfg.rope_theta <= 0 and cfg.max_position == 1024
+    eng = Engine("tiny-gpt2", device="cpu", max_batch=1, max_seq_len=4096)
+    assert eng.max_seq_len == cfg.max_position
+    r = eng.submit(list(range(1, 3001)), SamplingParams(max_new_tokens=50))
+    assert len(r.prompt_ids) == cfg.max_position - 1 and r.params.max_new_tokens == 1
+    assert Engine("tiny-llama", device="cpu", max_batch=1, max_seq_len=4096).max_seq_len == 4096
+    with pytest.raises(ValueError, match="learned positions"):
+        GpuRunner(cfg, "", 0, 1, torch.device("cuda:0"), max_batch=1, max_seq_len=cfg.max_position + 1)
+
+
 def test_engine_cancel_frees_slot_and_pages():
     """ADVICE r1: an abandoned request (stop word / disconnect / timeout) must not decode to max_new_tokens"""
     eng = Engine("tiny-llama", device="cpu", max_batch=1, max_seq_len=256, decode_burst=2)
