@@ -23,6 +23,7 @@ from fastapi.security import APIKeyHeader
 from pydantic import BaseModel
 
 from .p2p_runtime import P2PNode
+from .services import sampling_filters
 from .utils import now_ms
 
 try:
@@ -103,6 +104,8 @@ class ChatRequest(BaseModel):
     max_new_tokens: Optional[int] = None
     temperature: Optional[float] = 0.7
     stream: Optional[bool] = False
+    top_k: Optional[int] = None       # keep the k most likely tokens; absent = off
+    min_p: Optional[float] = None     # keep tokens with p >= min_p * p_max; absent = off
 
 
 @app.get("/")
@@ -205,6 +208,8 @@ async def chat(req: ChatRequest):
         return {"status": "error", "message": "node not started"}
     params = {"prompt": req.prompt, "max_new_tokens": req.max_new_tokens or 2048,
               "temperature": 0.7 if req.temperature is None else req.temperature}
+    filters = sampling_filters({"top_k": req.top_k, "min_p": req.min_p})
+    params.update(filters)
     try:
         t0 = time.time()
         want_local = req.provider_id in (None, "local", node.peer_id)
@@ -235,7 +240,7 @@ async def chat(req: ChatRequest):
                 try:
                     await node.request_generation(pid, req.prompt, params["max_new_tokens"], req.model,
                                                   temperature=params["temperature"], stream=True,
-                                                  on_chunk=q.put_nowait)
+                                                  on_chunk=q.put_nowait, **filters)
                 finally:
                     q.put_nowait(None)
 
@@ -254,7 +259,7 @@ async def chat(req: ChatRequest):
 
             return StreamingResponse(body(), media_type="text/plain")
         result = await node.request_generation(pid, req.prompt, params["max_new_tokens"], req.model,
-                                               temperature=params["temperature"])
+                                               temperature=params["temperature"], **filters)
         return {"status": "ok", "text": result.get("text", ""), "rid": f"p2p-{now_ms()}",
                 "metadata": {"engine": "coithub-p2p", "node": pid,
                              "latency_ms": result.get("latency_ms", int((time.time() - t0) * 1000))}}

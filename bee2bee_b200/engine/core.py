@@ -37,6 +37,8 @@ class SamplingParams:
     temperature: float = 0.7
     top_p: float = 0.95                # reference streaming default (hf.py:103)
     repetition_penalty: float = 1.15   # reference streaming default (hf.py:95)
+    top_k: int = 0                     # keep the k most likely tokens (ties kept) before top-p; 0 = off
+    min_p: float = 0.0                 # after top-p keep tokens with p >= min_p * p_max; 0 = off
     seed: Optional[int] = None
     stop_token_ids: Sequence[int] = ()
     ignore_eos: bool = False
@@ -108,7 +110,7 @@ class TorchRunner:
         seen = torch.zeros(1, V, dtype=torch.bool)
         seen[0, torch.tensor(sorted(st["seen"]), dtype=torch.long)] = True
         tok = int(sample_reference(logits[None, :V].cpu(), seen, st["temperature"], st["top_p"], st["rep"],
-                                   st["gen"]))
+                                   st["gen"], top_k=st["top_k"], min_p=st["min_p"]))
         st["seen"].add(tok)
         return tok
 
@@ -117,7 +119,8 @@ class TorchRunner:
             for s in seqs:
                 self.cache.pop(s.slot, None)
                 g = torch.Generator().manual_seed(int(s.seed) & 0x7FFFFFFF)
-                st = dict(temperature=s.temperature, top_p=s.top_p, rep=s.repetition_penalty, gen=g,
+                st = dict(temperature=s.temperature, top_p=s.top_p, rep=s.repetition_penalty, top_k=s.top_k,
+                          min_p=s.min_p, gen=g,
                           seen=set(int(t) for t in s.prompt), pos=len(s.prompt), hist=[])
                 logits = self._forward(s.slot, list(s.prompt), 0)
                 tok = self._sample(st, logits)
@@ -223,6 +226,10 @@ class Engine:
     def submit(self, prompt_ids: Sequence[int], params: Optional[SamplingParams] = None,
                on_token: Optional[Callable[[int], None]] = None) -> Request:
         params = params or SamplingParams()
+        if not params.top_k >= 0:
+            raise ValueError(f"top_k must be >= 0 (0 = off), got {params.top_k}")
+        if not 0.0 <= params.min_p <= 1.0:
+            raise ValueError(f"min_p must lie in [0, 1] (0 = off), got {params.min_p}")
         ids = list(prompt_ids)[-(self.max_seq_len - 1):] or [max(self.cfg.bos_token_id, 0)]
         budget = self.max_seq_len - len(ids)
         if params.max_new_tokens > budget:
@@ -414,7 +421,9 @@ class Engine:
             seqs = [SeqInit(slot=r.slot, prompt=r.prompt_ids, pages=self.alloc.owned(r.slot),
                             temperature=r.params.temperature, top_p=r.params.top_p,
                             repetition_penalty=r.params.repetition_penalty,
-                            seed=r.params.seed if r.params.seed is not None else (r.rid * 2654435761) & 0x7FFFFFFF,
+                            # k >= vocab already means off; the clamp keeps any k a client sends inside int32
+                            top_k=min(int(r.params.top_k), self.cfg.vocab_size),
+                            min_p=r.params.min_p, seed=r.params.seed if r.params.seed is not None else (r.rid * 2654435761) & 0x7FFFFFFF,
                             cached=self.alloc.cached_tokens(r.slot))
                     for r in admitted]
             for r in admitted:          # after the whole admission round: requests of one round never share with each other

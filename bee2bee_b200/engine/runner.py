@@ -43,6 +43,8 @@ class SeqInit:
     temperature: float = 0.7
     top_p: float = 0.95
     repetition_penalty: float = 1.15
+    top_k: int = 0           # 0 = off
+    min_p: float = 0.0       # 0 = off
     seed: int = 0
     cached: int = 0          # leading prompt tokens whose KV is already resident in ``pages`` (prefix cache): not prefilled
 
@@ -139,6 +141,8 @@ class GpuRunner:
         self.q_start = torch.arange(self.gb, device=dev, dtype=i32)
         self.temperature = torch.zeros(B, device=dev)
         self.top_p = torch.ones(B, device=dev)
+        self.top_k = torch.zeros(B, device=dev, dtype=i32)
+        self.min_p = torch.zeros(B, device=dev)
         self.rep_pen = torch.ones(B, device=dev)
         self.seeds = torch.zeros(B, device=dev, dtype=i32)
         self.hist_pos = torch.zeros(B, device=dev, dtype=i32)
@@ -242,18 +246,23 @@ class GpuRunner:
         for i, s in enumerate(seqs):
             bt_np[i, :len(s.pages)] = s.pages
         bt_host = torch.from_numpy(bt_np)
-        fl_host = torch.tensor([[s.temperature, s.top_p, s.repetition_penalty] for s in seqs], dtype=torch.float32)
-        seed_host = torch.tensor([int(s.seed) & 0x7FFFFFFF for s in seqs], dtype=i32)
+        fl_host = torch.tensor([[s.temperature, s.top_p, s.repetition_penalty, s.min_p] for s in seqs],
+                               dtype=torch.float32)
+        # seed and top_k in one int32 copy
+        int_host = torch.tensor([[int(s.seed) & 0x7FFFFFFF, int(s.top_k)] for s in seqs], dtype=i32)
         rows = torch.tensor([s.slot for s in seqs], dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
         fl = fl_host.pin_memory().to(dev, non_blocking=True)
+        iv = int_host.pin_memory().to(dev, non_blocking=True)
         self.block_table.index_copy_(0, rows, bt_host.pin_memory().to(dev, non_blocking=True))
         self.temperature.index_copy_(0, rows, fl[:, 0].contiguous())
         self.top_p.index_copy_(0, rows, fl[:, 1].contiguous())
         self.rep_pen.index_copy_(0, rows, fl[:, 2].contiguous())
-        self.seeds.index_copy_(0, rows, seed_host.pin_memory().to(dev, non_blocking=True))
+        self.min_p.index_copy_(0, rows, fl[:, 3].contiguous())
+        self.seeds.index_copy_(0, rows, iv[:, 0].contiguous())
+        self.top_k.index_copy_(0, rows, iv[:, 1].contiguous())
         self.hist_pos.index_fill_(0, rows, 0)
         self.seen.index_fill_(0, rows, 0)
-        self.h2d_bytes += bt_host.numel() * 4 + fl_host.numel() * 4 + S * (4 + 8)
+        self.h2d_bytes += bt_host.numel() * 4 + fl_host.numel() * 4 + int_host.numel() * 4 + S * 8
         if self.last:
             flat = np.concatenate([np.asarray(s.prompt, dtype=np.int32) for s in seqs])
             owner = np.repeat(np.asarray([s.slot for s in seqs], dtype=np.int32), [len(s.prompt) for s in seqs])
@@ -333,7 +342,8 @@ class GpuRunner:
             if self.last:
                 multi = self.world > 1
                 ops.sample(out, self.tok_local if multi else self.tokens, seen=self.seen, temperature=self.temperature,
-                           top_p=self.top_p, rep_penalty=self.rep_pen, seeds=self.seeds, step=self.step_ctr,
+                           top_p=self.top_p, top_k=self.top_k, min_p=self.min_p, rep_penalty=self.rep_pen,
+                           seeds=self.seeds, step=self.step_ctr,
                            vocab=self.cfg.vocab_size, softcap=self.cfg.final_softcap,
                            history=self.mesh.hist_base() if multi else self.history.data_ptr(), hist_pos=self.hist_pos,
                            hist_stride=self.hist_len, peer_tokens=self.mesh.tok_base() if multi else 0,
@@ -429,7 +439,8 @@ class GpuRunner:
             hist_ptr = (self.mesh.history_ptr(g) if multi else self._grp(self.history, g).data_ptr())
             ops.sample(out, self._grp(self.tok_local, g) if multi else self._grp(self.tokens, g),
                        seen=self._grp(self.seen, g), temperature=self._grp(self.temperature, g),
-                       top_p=self._grp(self.top_p, g), rep_penalty=self._grp(self.rep_pen, g),
+                       top_p=self._grp(self.top_p, g), top_k=self._grp(self.top_k, g),
+                       min_p=self._grp(self.min_p, g), rep_penalty=self._grp(self.rep_pen, g),
                        seeds=self._grp(self.seeds, g), step=self.step_ctr, vocab=self.cfg.vocab_size,
                        softcap=self.cfg.final_softcap, history=hist_ptr, hist_pos=self._grp(self.hist_pos, g),
                        hist_stride=self.hist_len, peer_tokens=hand.out_x if multi else 0,

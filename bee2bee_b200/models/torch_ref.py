@@ -136,10 +136,13 @@ class TorchPiece:
 
 
 def sample_reference(logits: torch.Tensor, seen: Optional[torch.Tensor], temperature: float, top_p: float,
-                     rep_penalty: float, generator: Optional[torch.Generator] = None) -> torch.Tensor:
-    """HF-processor semantics (repetition penalty -> temperature -> top-p -> multinomial /
+                     rep_penalty: float, generator: Optional[torch.Generator] = None, top_k: int = 0,
+                     min_p: float = 0.0) -> torch.Tensor:
+    """HF-processor semantics (repetition penalty -> temperature -> top-k -> top-p -> min-p -> multinomial /
     greedy when temperature <= 0), cf. /root/reference/bee2bee/hf.py:91-105.
-    logits [B, V] fp32; seen [B, V] bool of ids already in the context."""
+    logits [B, V] fp32; seen [B, V] bool of ids already in the context.  ``top_k`` keeps the tokens at least as likely
+    as the k-th (ties kept; <= 0 or >= V = off); top-p then sees the top-k survivors renormalised; ``min_p`` keeps
+    p >= min_p * p_max (<= 0 = off)."""
     l = logits.float().clone()
     if seen is not None and rep_penalty != 1.0:
         pen = torch.where(l > 0, l / rep_penalty, l * rep_penalty)
@@ -147,12 +150,18 @@ def sample_reference(logits: torch.Tensor, seen: Optional[torch.Tensor], tempera
     if not temperature > 0:
         return l.argmax(-1)
     l = l / temperature
+    if 0 < top_k < l.shape[-1]:
+        kth = torch.topk(l, top_k, dim=-1).values[..., -1:]
+        l = l.masked_fill(l < kth, float("-inf"))
     if top_p < 1.0:
         sl, si = torch.sort(l, descending=False)
         cum = sl.softmax(-1).cumsum(-1)
         remove = cum <= (1 - top_p)
         remove[..., -1:] = False
         l = l.masked_fill(remove.scatter(1, si, remove), float("-inf"))
+    if min_p > 0.0:
+        p = l.softmax(-1)
+        l = l.masked_fill(p < min(min_p, 1.0) * p.amax(-1, keepdim=True), float("-inf"))
     return torch.multinomial(l.softmax(-1), 1, generator=generator).squeeze(-1)
 
 

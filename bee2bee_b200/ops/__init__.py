@@ -396,11 +396,13 @@ def get_attn_tc_min_q() -> int:
 # ---------------------------------------------------------------------- sampler
 def sample(logits, out_tokens, *, seen=None, temperature=None, top_p=None, rep_penalty=None, seeds=None, step=None,
            peer_tokens=0, history=0, hist_pos=None, hist_stride=0, signal_flag=0, signal_epoch=0, done_counter=0,
-           vocab=0, softcap=0.0, row_map=0):
-    """``row_map``: device address of int32 [rows of logits] mapping each logits row to its batch row (< 0 = skip)."""
+           vocab=0, softcap=0.0, row_map=0, top_k=None, min_p=None):
+    """``row_map``: device address of int32 [rows of logits] mapping each logits row to its batch row (< 0 = skip).
+    ``top_k`` (int32, <= 0 or >= vocab = off) and ``min_p`` (fp32, <= 0 = off) hold one entry per batch row, like
+    ``temperature``; None turns the filter off for every row."""
     native().sample(logits, seen, out_tokens, peer_tokens, history, hist_pos, hist_stride, vocab, softcap,
                     temperature, top_p,
-                    rep_penalty, seeds, step, signal_flag, signal_epoch, done_counter, row_map)
+                    rep_penalty, seeds, step, signal_flag, signal_epoch, done_counter, row_map, top_k, min_p)
     return out_tokens
 
 

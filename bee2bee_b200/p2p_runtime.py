@@ -27,7 +27,7 @@ from .dht import DHTNode, announce_piece
 from .p2p import generate_join_link, parse_join_link, registration_url, sha256_hex_bytes
 from .pieces import LayerPiece, piece_hashes, split_pieces, verify_and_reassemble
 from .registry import RegistryClient
-from .services import BaseService, ServiceError, build_service
+from .services import BaseService, ServiceError, build_service, sampling_filters
 from .transport import Connection, ConnectionClosed, InProcHub, WSServer, connect, ws_listen
 from .utils import get_lan_ip, get_public_ip, get_system_metrics, new_id, now_ms, offline, sha256_hex
 
@@ -469,7 +469,7 @@ class P2PNode:
         model = data.get("model")
         params = {"prompt": data.get("prompt"),
                   "max_new_tokens": int(data.get("max_new_tokens") or data.get("max_tokens") or 2048),
-                  "temperature": data.get("temperature", 0.7)}
+                  "temperature": data.get("temperature", 0.7), **sampling_filters(data)}
         svc = self._find_local_service(data.get("svc", "hf"), model)
         if svc is not None:
             # run as a task so this peer's reader keeps draining pings / other requests
@@ -509,7 +509,7 @@ class P2PNode:
     async def _relay(self, conn: Connection, rid: str, pid: str, params: Dict[str, Any], model: Optional[str]) -> None:
         try:
             res = await self.request_generation(pid, params["prompt"], params["max_new_tokens"], model,
-                                                temperature=params.get("temperature", 0.7))
+                                                temperature=params.get("temperature", 0.7), **sampling_filters(params))
             await self._send(conn, P.msg(P.GEN_RESULT, rid=rid, **res))
         except Exception as exc:
             await self._send(conn, P.msg(P.GEN_RESULT, rid=rid, error=f"relay_link_failure: {exc}"))
@@ -674,8 +674,11 @@ class P2PNode:
     async def request_generation(self, provider_id: str, prompt: str, max_new_tokens: int = 32,
                                  model_name: Optional[str] = None, temperature: float = 0.7, stream: bool = False,
                                  on_chunk: Optional[Callable[[str], None]] = None,
-                                 timeout: float = DEFAULT_GEN_TIMEOUT) -> Dict[str, Any]:
-        params = {"prompt": prompt, "max_new_tokens": max_new_tokens, "temperature": temperature}
+                                 timeout: float = DEFAULT_GEN_TIMEOUT, top_k: Optional[int] = None,
+                                 min_p: Optional[float] = None) -> Dict[str, Any]:
+        """``top_k`` / ``min_p``: optional sampling filters (None = off), passed on only when set."""
+        filters = sampling_filters({"top_k": top_k, "min_p": min_p})
+        params = {"prompt": prompt, "max_new_tokens": max_new_tokens, "temperature": temperature, **filters}
         if provider_id == self.peer_id:
             svc = self._find_local_service(None, model_name)
             if svc is None:
@@ -711,7 +714,7 @@ class P2PNode:
         try:
             ok = await self._send(conn, P.gen_request(rid, prompt, model=model_name, svc=svc_name,
                                                       max_new_tokens=max_new_tokens, temperature=temperature,
-                                                      stream=bool(stream or on_chunk)))
+                                                      stream=bool(stream or on_chunk), **filters))
             if not ok:
                 raise ConnectionError(f"send to {provider_id} failed")
             res = await asyncio.wait_for(fut, timeout)

@@ -27,7 +27,7 @@ from ..engine.tokenizer import STOP_WORDS, cut_at_stop_words, load_tokenizer, pa
 from ..models.config import ModelConfig, resolve_config, split_layers
 from ..models.torch_ref import TorchPiece, sample_reference
 from ..models.weights import load_or_init
-from ..services import BaseService, ServiceError
+from ..services import BaseService, ServiceError, sampling_filters
 from ..utils import new_id
 
 _DT = {"float32": torch.float32, "bfloat16": torch.bfloat16, "float16": torch.float16, "int64": torch.int64}
@@ -129,7 +129,8 @@ class MeshPipelineService(BaseService):
                 pass
 
     async def agenerate(self, prompt_ids: List[int], max_new: int, temperature: float, top_p: float = 1.0,
-                        rep: float = 1.0, on_token=None, seed: int = 0) -> List[int]:
+                        rep: float = 1.0, on_token=None, seed: int = 0, top_k: int = 0,
+                        min_p: float = 0.0) -> List[int]:
         session = new_id("sess")
         gen = torch.Generator().manual_seed(seed)
         seen = set(prompt_ids)
@@ -142,7 +143,8 @@ class MeshPipelineService(BaseService):
             for step in range(max_new):
                 seen_mask = torch.zeros(1, V, dtype=torch.bool)
                 seen_mask[0, torch.tensor(sorted(seen), dtype=torch.long)] = True
-                tok = int(sample_reference(logits[0, -1:, :V], seen_mask, temperature, top_p, rep, gen))
+                tok = int(sample_reference(logits[0, -1:, :V], seen_mask, temperature, top_p, rep, gen, top_k=top_k,
+                                           min_p=min_p))
                 out.append(tok)
                 seen.add(tok)
                 if on_token is not None:
@@ -167,7 +169,7 @@ class MeshPipelineService(BaseService):
         prompt, max_new, temperature = self._params(params)
         t0 = time.time()
         ids = self.tokenizer.encode(prompt)
-        out = await self.agenerate(ids, max_new, temperature)
+        out = await self.agenerate(ids, max_new, temperature, **sampling_filters(params))
         text = prompt + self.tokenizer.decode(out)
         return {"text": text, "tokens": len(out), "latency_ms": int((time.time() - t0) * 1000),
                 "price_per_token": self.price_per_token, "cost": self.price_per_token * len(out)}
@@ -178,7 +180,8 @@ class MeshPipelineService(BaseService):
             rendered = self.tokenizer.apply_chat_template(parse_transcript(prompt), add_generation_prompt=True)
             ids = self.tokenizer.encode(rendered)
             q: asyncio.Queue = asyncio.Queue()
-            task = asyncio.create_task(self.agenerate(ids, max_new, temperature, 0.95, 1.15, on_token=q.put_nowait))
+            task = asyncio.create_task(self.agenerate(ids, max_new, temperature, 0.95, 1.15, on_token=q.put_nowait,
+                                                      **sampling_filters(params)))
             toks: List[int] = []
             sent = ""
             while not (task.done() and q.empty()):

@@ -76,11 +76,18 @@ def service_announce(service: str, meta: Dict[str, Any]) -> Dict[str, Any]:
 
 
 def gen_request(rid: str, prompt: str, model: Optional[str] = None, svc: str = "hf", max_new_tokens: int = 2048,
-                temperature: float = 0.7, stream: bool = False) -> Dict[str, Any]:
+                temperature: float = 0.7, stream: bool = False, top_k: Optional[int] = None,
+                min_p: Optional[float] = None) -> Dict[str, Any]:
     # both spellings are sent: the reference reads ``max_tokens`` but its requester writes
     # ``max_new_tokens`` (p2p_runtime.py:577 vs 822)
-    return msg(GEN_REQUEST, rid=rid, prompt=prompt, model=model, svc=svc, max_new_tokens=max_new_tokens,
-               max_tokens=max_new_tokens, temperature=temperature, stream=stream)
+    m = msg(GEN_REQUEST, rid=rid, prompt=prompt, model=model, svc=svc, max_new_tokens=max_new_tokens,
+            max_tokens=max_new_tokens, temperature=temperature, stream=stream)
+    # optional sampling filters travel only when set, so a request without them is the reference's message
+    if top_k is not None:
+        m["top_k"] = int(top_k)
+    if min_p is not None:
+        m["min_p"] = float(min_p)
+    return m
 
 
 def request_id_of(m: Dict[str, Any]) -> Optional[str]:

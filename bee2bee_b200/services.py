@@ -33,6 +33,16 @@ class ServiceError(Exception):
     pass
 
 
+def sampling_filters(params: Dict[str, Any]) -> Dict[str, Any]:
+    """The ``top_k`` / ``min_p`` a request sets (absent or null = off), as keyword arguments."""
+    out: Dict[str, Any] = {}
+    if params.get("top_k") is not None:
+        out["top_k"] = int(params["top_k"])
+    if params.get("min_p") is not None:
+        out["min_p"] = float(params["min_p"])
+    return out
+
+
 class BaseService:
     def __init__(self, name: str):
         self.name = name
@@ -141,7 +151,7 @@ class HFService(BaseService):
             from .hf import generate_text
 
             text, ids = generate_text(self.model, self.tokenizer, self.device, prompt, max_new, temperature=temperature,
-                                      return_ids=True)
+                                      return_ids=True, **sampling_filters(params))
             n = len(ids)                       # exact count (the reference re-encodes text to estimate it)
             return {"text": text, "tokens": n, "latency_ms": int((time.time() - t0) * 1000.0),
                     "price_per_token": self.price_per_token, "cost": self.price_per_token * n}
@@ -155,7 +165,8 @@ class HFService(BaseService):
             prompt, max_new, temperature = self._args(params)
             from .hf import generate_text_stream
 
-            for delta in generate_text_stream(self.model, self.tokenizer, self.device, prompt, max_new, temperature):
+            for delta in generate_text_stream(self.model, self.tokenizer, self.device, prompt, max_new, temperature,
+                                              **sampling_filters(params)):
                 yield json.dumps({"text": delta}) + "\n"
             yield json.dumps({"done": True}) + "\n"
         except Exception as exc:
@@ -190,9 +201,12 @@ class EmbeddedOllama:
 
         lm = self._ensure()
         opts = payload.get("options") or {}
+        # top_k / min_p only when the request sets them: Ollama's own top_k default (40) is not applied.  Ollama (like
+        # llama.cpp) treats top_k <= 0 and min_p <= 0 as off, so negative values mean off here too.
+        filters = {k: v if v > 0 else type(v)(0) for k, v in sampling_filters(opts).items()}
         sp = SamplingParams(max_new_tokens=int(opts.get("num_predict", 128)),
                             temperature=float(opts.get("temperature", 0.8)), top_p=float(opts.get("top_p", 0.9)),
-                            repetition_penalty=float(opts.get("repeat_penalty", 1.1)))
+                            repetition_penalty=float(opts.get("repeat_penalty", 1.1)), **filters)
         ids = self._tok.encode(payload.get("prompt", ""))
         t0 = time.time()
         import queue as _q
@@ -278,7 +292,7 @@ class OllamaService(BaseService):
             raise ServiceError("Missing prompt")
         return {"model": self.actual_model, "prompt": prompt, "stream": stream,
                 "options": {"num_predict": int(params.get("max_new_tokens") or params.get("max_tokens") or 2048),
-                            "temperature": float(params.get("temperature", 0.7) or 0.7)}}
+                            "temperature": float(params.get("temperature", 0.7) or 0.7), **sampling_filters(params)}}
 
     def execute(self, params: Dict[str, Any]) -> Dict[str, Any]:
         payload = self._payload(params, stream=False)

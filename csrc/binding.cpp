@@ -377,8 +377,22 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
             int64_t history, const OptT& hist_pos, int64_t hist_stride, int64_t vocab, double softcap,
             const OptT& temperature, const OptT& top_p,
             const OptT& rep_penalty, const OptT& seeds, const OptT& step, int64_t signal_flag, int64_t signal_epoch,
-            int64_t done_counter, int64_t row_map) {
+            int64_t done_counter, int64_t row_map, const OptT& top_k, const OptT& min_p) {
   TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.stride(1) == 1, "logits: fp32");
+  // top_k / min_p are per-sequence state like temperature: one entry per state row (logits row b reads row
+  // row_map[b], or b without a row_map)
+  const bool has_temp = temperature.has_value() && temperature->defined();
+  const int64_t state_rows = has_temp ? temperature->numel() : logits.size(0);
+  auto check_row_param = [&](const OptT& t, at::ScalarType dtype, const char* name) {
+    if (!(t.has_value() && t->defined())) return;
+    TORCH_CHECK(t->scalar_type() == dtype && t->device() == logits.device() && t->dim() == 1 && t->is_contiguous(),
+                name, " must be a contiguous 1-D ", dtype == at::kInt ? "int32" : "float32",
+                " tensor on the logits' device");
+    TORCH_CHECK(t->numel() == state_rows && (row_map != 0 || t->numel() >= logits.size(0)), name, " has ", t->numel(),
+                " entries; expected one per state row (", state_rows, ")");
+  };
+  check_row_param(top_k, at::kInt, "top_k");
+  check_row_param(min_p, at::kFloat, "min_p");
   c10::cuda::CUDAGuard guard(logits.device());
   int* hp = ptr_or_null<int>(hist_pos);
   check(b2b::launch_sample(reinterpret_cast<const float*>(logits.data_ptr()), ptr_or_null<uint32_t>(seen),
@@ -390,7 +404,7 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
                            ptr_or_null<const float>(rep_penalty), ptr_or_null<const uint32_t>(seeds),
                            ptr_or_null<const uint32_t>(step), as_ptr<uint32_t>(signal_flag),
                            as_ptr<uint32_t>(signal_epoch), as_ptr<uint32_t>(done_counter), as_ptr<const int>(row_map),
-                           cur_stream()),
+                           ptr_or_null<const int>(top_k), ptr_or_null<const float>(min_p), cur_stream()),
         "sample");
 }
 

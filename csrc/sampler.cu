@@ -1,12 +1,26 @@
-// Fused sampler for sm_90a: repetition penalty (seen-token bitmap) -> temperature ->
-// exact top-p via two-level radix histogram of the probability bits -> multinomial draw
-// (or argmax when temperature <= 0).  One CTA per sequence, logits are fp32 [B, ld] as
-// written by the lm_head GEMM.  The sampled id is stored locally (token ring, history
-// bitmap) and, on the last piece of a pipeline, straight into piece 0's token buffer on
+// Fused sampler for sm_90a: repetition penalty (seen-token bitmap) -> temperature -> top-k ->
+// top-p -> min-p, each decided on a two-level radix histogram of the probability bits ->
+// multinomial draw (or argmax when temperature <= 0).  One cluster per sequence, logits are
+// fp32 [B, ld] as written by the lm_head GEMM.  The sampled id is stored locally (token ring,
+// history bitmap) and, on the last piece of a pipeline, straight into piece 0's token buffer on
 // the peer GPU followed by a release flag (4 bytes/sequence over NVLink, no NCCL).
 //
 // Semantics follow the reference's generation defaults (bee2bee/hf.py:91-105):
 // repetition_penalty 1.15, top_p 0.95, do_sample iff temperature > 0, greedy otherwise.
+// After temperature the filters run in transformers' processor order, with e = exp(l - max):
+//   * top-k (k per row; k <= 0 or k >= V = off): K = the tokens whose e is at least the k-th
+//     largest e, ties at the k-th value kept.  K is decided on the same 22-bit key (top 22 bits
+//     of the 28-bit key below) as top-p, so it may also keep tokens whose e lies within one
+//     level-2 bin (a relative 2^-18 to 2^-17) below the k-th, and every token with e < 2^-32
+//     when the k-th is below 2^-32;
+//   * top-p over K: need = min(top_p, 1) Z_K with Z_K the mass of K; the nucleus is the smallest
+//     highest-e prefix reaching need (a prefix of K, so it is found on the unchanged mass
+//     histograms);
+//   * min-p (per row; <= 0 = off): keep e >= min(min_p, 1) on the full 28-bit key, i.e.
+//     p >= min_p p_max.
+// Every filter keeps a highest-e prefix, so the kept set is {key >= max(thr_k, thr_p, key(min_p))}
+// and always holds the maximal tokens.  Greedy rows ignore top-k and min-p.  The branches on
+// top-k and min-p are uniform per row: a row with both off runs the phases of plain top-p.
 //
 // Performance notes: every pass over the 128k logits is
 // L2-latency bound, so logits are read 8 at a time per thread (2 x 128-bit loads in flight);
@@ -41,6 +55,8 @@ struct SampleParams {
   float softcap;            // final-logit soft-capping (Gemma-2), 0 = off
   const float* temperature; // [rows]
   const float* top_p;       // [rows]
+  const int* top_k;         // [rows] (<= 0 or >= vocab = off), or null
+  const float* min_p;       // [rows] (<= 0 = off), or null
   const float* rep_penalty; // [rows]
   const uint32_t* seeds;    // [rows]
   const uint32_t* step;     // device step counter (rng stream), may be null
@@ -69,6 +85,7 @@ struct __align__(16) SampShared {
   unsigned long long wsum[32];
   unsigned long long red_u[32];
   unsigned long long cz[MAX_CS];            // per-CTA partition-function partials (written by every peer)
+  unsigned long long czk[MAX_CS];           // per-CTA partials of Z_K, the mass of the top-k set
   float cmax[MAX_CS];
   int camx[MAX_CS];
   float ctot[MAX_CS];                       // per-CTA kept mass
@@ -94,6 +111,9 @@ __device__ __forceinline__ void hist_add(uint32_t* lo, uint32_t* hi, int bin, ui
   const uint32_t old = atomicAdd(&lo[bin], f);
   if (old + f < old) atomicAdd(&hi[bin], 1u);
 }
+// histogram kind for merge_and_find: 32.32 fixed-point mass in two words, or a 32-bit token count in one
+template <bool C>
+struct CountHist { static constexpr bool value = C; };
 
 // One CLUSTER of CS CTAs per sequence (grid = [B, 1, CS]); CTA r owns ids [r*W, (r+1)*W).  A single
 // SM is instruction-bound on a 128k vocabulary, so the
@@ -273,16 +293,23 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
 
   // cluster-wide histogram -> S.merged (every CTA computes the same sum), then a top-down search for the
   // highest bin whose suffix mass (plus `carry`) reaches `need`.  Results: s_i[0] = bin, s_u[0] = mass above it.
-  auto merge_and_find = [&](uint32_t* hlo, uint32_t* hhi, unsigned long long carry, unsigned long long need) {
+  // `kind` is CountHist<true> for a count histogram in `hlo` alone (then the suffix is a token count).
+  auto merge_and_find = [&](auto kind, const uint32_t* hlo, const uint32_t* hhi, unsigned long long carry,
+                            unsigned long long need) {
     {
       const int bin = 2 * tid;        // SBINS == 2 * SAMP_THREADS
       unsigned long long m0 = 0ull, m1 = 0ull;
-      const uint32_t alo = smem_u32(&hlo[bin]), ahi = smem_u32(&hhi[bin]);
+      const uint32_t alo = smem_u32(&hlo[bin]);
       for (int c = 0; c < CS; ++c) {
         const uint2 l2 = ld_dsmem_v2u32(mapa_smem(alo, c));
-        const uint2 h2 = ld_dsmem_v2u32(mapa_smem(ahi, c));
-        m0 += (static_cast<unsigned long long>(h2.x) << 32) | l2.x;
-        m1 += (static_cast<unsigned long long>(h2.y) << 32) | l2.y;
+        if constexpr (decltype(kind)::value) {
+          m0 += l2.x;
+          m1 += l2.y;
+        } else {
+          const uint2 h2 = ld_dsmem_v2u32(mapa_smem(smem_u32(&hhi[bin]), c));
+          m0 += (static_cast<unsigned long long>(h2.x) << 32) | l2.x;
+          m1 += (static_cast<unsigned long long>(h2.y) << 32) | l2.y;
+        }
       }
       S.merged[bin] = m0; S.merged[bin + 1] = m1;
       unsigned long long ws = m0 + m1;      // warp w covers bins [64w, 64w + 64)
@@ -326,8 +353,50 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
 
   unsigned long long Z = 0ull;
   for (int c = 0; c < CS; ++c) Z += S.cz[c];
+
+  // ---- top-k (row-uniform): the 22-bit key prefix thr_k of the k-th largest e from two count levels, then
+  // Z = Z_K, the mass of {key >= thr_k}.  The level-2 arrays are idle until phase 3 and hold the counts.
+  const int top_k = p.top_k ? p.top_k[bb] : 0;
+  if (top_k > 0 && top_k < V) {
+    for (int j = tid; j < n; j += SAMP_THREADS) atomicAdd(&S.h2_lo[dkey(ebuf[j]) >> 17], 1u);
+    __syncthreads();
+    cluster_sync_all();
+    merge_and_find(CountHist<true>{}, S.h2_lo, nullptr, 0ull, static_cast<unsigned long long>(top_k));
+    const int K1 = S.s_i[0];
+    const unsigned long long above_k = S.s_u[0];      // tokens strictly above the boundary bin
+    __syncthreads();
+    for (int j = tid; j < n; j += SAMP_THREADS) {
+      const uint32_t d = dkey(ebuf[j]);
+      if (static_cast<int>(d >> 17) == K1) atomicAdd(&S.h2_hi[(d >> 6) & (SBINS - 1)], 1u);
+    }
+    __syncthreads();
+    cluster_sync_all();
+    merge_and_find(CountHist<true>{}, S.h2_hi, nullptr, above_k, static_cast<unsigned long long>(top_k));
+    const uint32_t thr_k = (static_cast<uint32_t>(K1) << 17) | (static_cast<uint32_t>(S.s_i[0]) << 6);
+    unsigned long long zk = 0ull;
+    for (int j = tid; j < n; j += SAMP_THREADS) {
+      const float e = ebuf[j];
+      if (dkey(e) >= thr_k) zk += fx32(e);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) zk += __shfl_xor_sync(0xffffffffu, zk, o);
+    if (lane == 0) S.red_u[warp] = zk;
+    __syncthreads();
+    if (warp == 0) {
+      unsigned long long z = S.red_u[lane];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+      if (lane < CS) st_dsmem_u64(mapa_smem(smem_u32(&S.czk[r]), lane), z);
+    }
+    cluster_sync_all();               // also: no peer reads this CTA's count histograms any more
+    Z = 0ull;
+    for (int c = 0; c < CS; ++c) Z += S.czk[c];
+    for (int i = tid; i < SBINS; i += SAMP_THREADS) { S.h2_lo[i] = 0u; S.h2_hi[i] = 0u; }
+    // the __syncthreads inside the level-1 search below orders these stores before phase 3
+  }
+
   const unsigned long long need = static_cast<unsigned long long>(static_cast<double>(top_p) * static_cast<double>(Z));
-  merge_and_find(S.h1_lo, S.h1_hi, 0ull, need);
+  merge_and_find(CountHist<false>{}, S.h1_lo, S.h1_hi, 0ull, need);
   const int B1 = S.s_i[0];
   const unsigned long long above1 = S.s_u[0];       // mass strictly above the boundary bin
   __syncthreads();                                   // s_i / merged are reused by the second level
@@ -351,8 +420,11 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
   }
   __syncthreads();
   cluster_sync_all();
-  merge_and_find(S.h2_lo, S.h2_hi, above1, need);
-  const uint32_t thr = (static_cast<uint32_t>(B1) << 17) | (static_cast<uint32_t>(S.s_i[0]) << 6);
+  merge_and_find(CountHist<false>{}, S.h2_lo, S.h2_hi, above1, need);
+  // the nucleus is a prefix of K (need <= Z_K), so thr >= thr_k; min-p (row-uniform) can only raise it
+  uint32_t thr = (static_cast<uint32_t>(B1) << 17) | (static_cast<uint32_t>(S.s_i[0]) << 6);
+  const float min_p = p.min_p ? p.min_p[bb] : 0.f;
+  if (min_p > 0.f) thr = max(thr, dkey(fminf(min_p, 1.f)));
 
   // ---- phase 4: multinomial draw over the kept set {dkey(e) >= thr}, in id order.
   // warp w owns a contiguous chunk of this CTA's slice; lanes own interleaved quads.
@@ -454,11 +526,12 @@ int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* pee
                   const int* hist_pos, int* hist_pos_out, int hist_stride, int batch, int vocab, int ld, float softcap,
                   const float* temperature, const float* top_p, const float* rep_penalty, const uint32_t* seeds,
                   const uint32_t* step, uint32_t* signal_flag, uint32_t* signal_epoch, uint32_t* done_counter,
-                  const int* row_map, cudaStream_t s) {
+                  const int* row_map, const int* top_k, const float* min_p, cudaStream_t s) {
   SampleParams p;
   p.logits = logits; p.seen = seen; p.out_tokens = out_tokens; p.peer_tokens = peer_tokens; p.history = history;
   p.hist_pos = hist_pos; p.hist_pos_out = hist_pos_out; p.hist_stride = hist_stride; p.vocab = vocab; p.ld = ld; p.softcap = softcap;
-  p.temperature = temperature; p.top_p = top_p; p.rep_penalty = rep_penalty; p.seeds = seeds; p.step = step;
+  p.temperature = temperature; p.top_p = top_p; p.top_k = top_k; p.min_p = min_p; p.rep_penalty = rep_penalty;
+  p.seeds = seeds; p.step = step;
   p.signal_flag = signal_flag; p.signal_epoch = signal_epoch; p.done_counter = done_counter; p.row_map = row_map;
   if (sample_cluster_size(1, vocab, 0) == 0) return -6;
   static int sm_count[64] = {};

@@ -1,22 +1,66 @@
-import os, sys
+"""Time ``sample`` at B=32, V=128256 (Llama-3 vocabulary), T=0.7, repetition penalty 1.15, for four filter settings:
+off (top_p 0.95), top_k=50, top_k=50 with top_p=0.95, and min_p=0.05.  The settings run in one process and alternate
+round by round, so clock and neighbour load drift hit all of them alike.  Prints the card and its power limit."""
+import os
+import subprocess
+import sys
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
+
 from bee2bee_b200 import ops
-B, V = 32, 128256
+
+B, V, ITERS, ROUNDS = 32, 128256, 50, 6
+dev = "cuda"
+try:
+    power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+except OSError:
+    power = "unknown"
+print(f"card: {torch.cuda.get_device_name()}  power limit: {power or 'unknown'}")
+
 torch.manual_seed(0)
-logits = torch.randn(B, V, device="cuda")
-out = torch.zeros(B, device="cuda", dtype=torch.int32)
-seen = torch.zeros(B, (V + 31) // 32, device="cuda", dtype=torch.int32)
-t = torch.full((B,), 0.7, device="cuda"); p = torch.full((B,), 0.95, device="cuda"); rp = torch.full((B,), 1.15, device="cuda")
-seeds = torch.arange(B, device="cuda", dtype=torch.int32); step = torch.zeros(1, device="cuda", dtype=torch.int32)
-for scale in (1.0, 4.0):
-    lg = logits * scale
-    for _ in range(3):
-        ops.sample(lg, out, seen=seen, temperature=t, top_p=p, rep_penalty=rp, seeds=seeds, step=step)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(20):
-        ops.sample(lg, out, seen=seen, temperature=t, top_p=p, rep_penalty=rp, seeds=seeds, step=step)
-    e1.record(); torch.cuda.synchronize()
-    print(f"sampler B={B} V={V} logit-scale {scale}: {e0.elapsed_time(e1)*1e3/20:.1f} us")
+logits = torch.randn(B, V, device=dev) * 4.0
+out = torch.zeros(B, device=dev, dtype=torch.int32)
+seen = torch.zeros(B, (V + 31) // 32, device=dev, dtype=torch.int32)
+seen[:, :64] = 0x01010101                       # some ids already in the context
+t = torch.full((B,), 0.7, device=dev)
+rp = torch.full((B,), 1.15, device=dev)
+seeds = torch.arange(B, device=dev, dtype=torch.int32)
+step = torch.zeros(1, device=dev, dtype=torch.int32)
+
+
+def full(v, dtype=torch.float32):
+    return torch.full((B,), v, device=dev, dtype=dtype)
+
+
+rows = {
+    "off (top_p 0.95)": dict(top_p=full(0.95)),
+    "top_k=50": dict(top_p=full(1.0), top_k=full(50, torch.int32), min_p=full(0.0)),
+    "top_k=50 top_p=0.95": dict(top_p=full(0.95), top_k=full(50, torch.int32), min_p=full(0.0)),
+    "min_p=0.05": dict(top_p=full(1.0), top_k=full(0, torch.int32), min_p=full(0.05)),
+}
+
+
+def call(kw):
+    ops.sample(logits, out, seen=seen, temperature=t, rep_penalty=rp, seeds=seeds, step=step, **kw)
+
+
+for kw in rows.values():
+    for _ in range(5):
+        call(kw)
+torch.cuda.synchronize()
+times = {name: [] for name in rows}
+for _ in range(ROUNDS):
+    for name, kw in rows.items():
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(ITERS):
+            call(kw)
+        e1.record()
+        torch.cuda.synchronize()
+        times[name].append(e0.elapsed_time(e1) * 1e3 / ITERS)
+for name, ts in times.items():
+    ts = sorted(ts)
+    print(f"sampler B={B} V={V} {name:22s}: median {ts[len(ts) // 2]:.1f} us  (min {ts[0]:.1f}, max {ts[-1]:.1f}, "
+          f"{ROUNDS} rounds x {ITERS} launches)")
