@@ -162,7 +162,8 @@ def pick_splitk(n_out: int, m_tok: int, k: int, bn: int, epi: int, stages: int =
     if (n_out, k) in SPLITK_OVERRIDE:
         want = SPLITK_OVERRIDE[(n_out, k)]
     else:
-        # up to ~2 CTAs per SM (Llama-3-8B decode, bn=32: qkv 4, o 4, gate/up 1, down 8; bn=16: 4/4/1/4); >= 16
+        # up to ~2 CTAs per SM at the default ring (Llama-3-8B decode, bn=32: qkv 4, o 4, gate/up 1, down 8; bn=16:
+        # 4/4/1/4; the launcher shortens the ring of a grid that would need a second wave, e.g. down at bn=32); >= 16
         # k-blocks per CTA, and every CTA of the cluster keeps >= 4 token columns
         tiles = (n_out // 128) * ((m_tok + bn - 1) // bn)
         limit = 256 if bn >= 32 else 200

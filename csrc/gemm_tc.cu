@@ -677,8 +677,65 @@ int make_tmap_shared(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t co
   return make_tmap(m, ptr, rows, cols, ld, box_rows, elt_bytes);
 }
 
+// CTAs of this instantiation that are resident at once with a `stages`-deep ring, in clusters of `splitk`, as the
+// driver counts them (clusters must fit inside a GPC, so this is not SMs x CTAs per SM).  Cached per (device, split-K,
+// depth); 0 if the driver cannot say.
 template <int BN, int EPI, int QM>
-static int launch_bn_epi(const GemmParams& p, const CUtensorMap& tw, const CUtensorMap& tx, cudaStream_t stream) {
+static int resident_ctas(int dev, int splitk, int stages) {
+  static std::map<std::tuple<int, int, int>, int> cache;
+  static std::mutex mu;
+  std::lock_guard<std::mutex> g(mu);
+  const std::tuple<int, int, int> key{dev, splitk, stages};
+  auto it = cache.find(key);
+  if (it != cache.end()) return it->second;
+  const int smem = GemmCfg<BN>::smem_bytes(stages);
+  int n = 0;
+  if (splitk > 1) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(1, 1, splitk);
+    cfg.blockDim = dim3(GEMM_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute attr{};
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 1;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = splitk;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    if (cudaOccupancyMaxActiveClusters(&clusters, gemm_tc_kernel<BN, EPI, QM>, &cfg) == cudaSuccess) n = clusters * splitk;
+    else cudaGetLastError();   // not a launch error: the caller keeps the default depth
+  } else {
+    int per_sm = 0, sms = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_tc_kernel<BN, EPI, QM>, GEMM_THREADS, smem) == cudaSuccess &&
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess)
+      n = per_sm * sms;
+    else cudaGetLastError();
+  }
+  cache[key] = n;
+  return n;
+}
+
+// Ring depth of a decode launch (one token tile) that asked for the tile's default: the default, unless its grid needs
+// more than one wave and a shallower ring (3 stages at least, still holding the split-K landing zone) lets the whole
+// grid be resident at once.  A partial second wave costs a whole CTA's time for a fraction of the weights (Llama-3-8B
+// down-projection at 32 tokens: 256 CTAs in clusters of 8, 56 -> 46 us per layer on an H100 with a 3-stage ring);
+// when a grid takes several waves at any depth (lm_head), the deeper ring streams faster.  The depth changes neither
+// the k-block order nor any sum, so the output is the same.
+template <int BN, int EPI, int QM>
+static int decode_depth(const GemmParams& p, int dev) {
+  const int ctas = (p.n_out / BM) * p.splitk;
+  if (resident_ctas<BN, EPI, QM>(dev, p.splitk, p.stages) >= ctas) return p.stages;
+  for (int st = p.stages - 1; st >= 3; --st) {
+    if (gemm_tc_max_splitk(BN, p.epi, st) < p.splitk) break;
+    if (resident_ctas<BN, EPI, QM>(dev, p.splitk, st) >= ctas) return st;
+  }
+  return p.stages;
+}
+
+template <int BN, int EPI, int QM>
+static int launch_bn_epi(const GemmParams& p_in, const CUtensorMap& tw, const CUtensorMap& tx, bool default_depth,
+                         cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set[64] = {};      // per device: one process may drive several GPUs (enable_peer_access path)
   int dev = 0;
@@ -689,6 +746,8 @@ static int launch_bn_epi(const GemmParams& p, const CUtensorMap& tw, const CUten
     if (e != cudaSuccess) return static_cast<int>(e);
     if (dev < 64) attr_set[dev] = true;
   }
+  GemmParams p = p_in;
+  if (default_depth && p.m_tok <= BN && QM != 2) p.stages = static_cast<int8_t>(decode_depth<BN, EPI, QM>(p, dev));
   return static_cast<int>(launch_kernel(gemm_tc_kernel<BN, EPI, QM>, dim3(p.n_out / BM, (p.m_tok + BN - 1) / BN, p.splitk),
                                         dim3(GEMM_THREADS), Cfg::smem_bytes(p.stages), stream, static_cast<unsigned>(p.splitk), tw, tx, p));
 }
@@ -696,14 +755,16 @@ static int launch_bn_epi(const GemmParams& p, const CUtensorMap& tw, const CUten
 // one compact kernel per (token tile, epilogue): a runtime `switch` inside the 16x-unrolled epilogue
 // loop would make the kernel instruction-fetch bound
 template <int BN>
-static int launch_bn(const GemmParams& p, const CUtensorMap& tw, const CUtensorMap& tx, cudaStream_t stream) {
+static int launch_bn(const GemmParams& p, const CUtensorMap& tw, const CUtensorMap& tx, bool default_depth,
+                     cudaStream_t stream) {
 #define B2B_EPI_CASE(E)                                                                              \
   case E:                                                                                            \
     if (p.fp8 && p.sfa != nullptr) {                                                                 \
-      if constexpr (BN >= 32) return launch_bn_epi<BN, E, 2>(p, tw, tx, stream);                     \
+      if constexpr (BN >= 32) return launch_bn_epi<BN, E, 2>(p, tw, tx, default_depth, stream);      \
       else return -7;   /* MX scale-factor chunks are laid out for token tiles of >= 32 */           \
     }                                                                                                \
-    return p.fp8 ? launch_bn_epi<BN, E, 1>(p, tw, tx, stream) : launch_bn_epi<BN, E, 0>(p, tw, tx, stream);
+    return p.fp8 ? launch_bn_epi<BN, E, 1>(p, tw, tx, default_depth, stream)                         \
+                 : launch_bn_epi<BN, E, 0>(p, tw, tx, default_depth, stream);
   switch (p.epi) {
     B2B_EPI_CASE(EPI_PLAIN)
     B2B_EPI_CASE(EPI_RESIDUAL)
@@ -801,6 +862,7 @@ int launch_gemm_tc(const GemmParams& p_in, const void* w, const void* x, int bn,
   const int elt = p.fp8 ? 1 : 2;
   const int bke = ROW_BYTES / elt;
   if (p.n_out % BM != 0 || p.k % bke != 0 || p.m_tok <= 0) return -2;
+  const bool default_depth = p_in.stages <= 0;
   {
     int stages = 0, splitk = 0;
     const int qm = p.fp8 ? (p.sfa != nullptr ? 2 : 1) : 0;
@@ -815,11 +877,11 @@ int launch_gemm_tc(const GemmParams& p_in, const void* w, const void* x, int bn,
   r = make_tmap(&tx, x, p.m_tok, p.k, p.k, bn, elt);
   if (r) return r;
   switch (bn) {
-    case 16: return launch_bn<16>(p, tw, tx, stream);
-    case 32: return launch_bn<32>(p, tw, tx, stream);
-    case 64: return launch_bn<64>(p, tw, tx, stream);
-    case 128: return launch_bn<128>(p, tw, tx, stream);
-    case 256: return launch_bn<256>(p, tw, tx, stream);
+    case 16: return launch_bn<16>(p, tw, tx, default_depth, stream);
+    case 32: return launch_bn<32>(p, tw, tx, default_depth, stream);
+    case 64: return launch_bn<64>(p, tw, tx, default_depth, stream);
+    case 128: return launch_bn<128>(p, tw, tx, default_depth, stream);
+    case 256: return launch_bn<256>(p, tw, tx, default_depth, stream);
     default: return -3;
   }
 }

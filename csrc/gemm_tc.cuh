@@ -94,7 +94,8 @@ int gemm_tc_max_splitk(int bn, int epi, int stages);
 // The (ring depth, cluster split-K) a launch with these arguments runs: `stages` <= 0 or above the tile's default ->
 // the default, then at least 2; `splitk` clamped to 1..8, to gemm_tc_max_splitk, to the number of k-blocks, then
 // rounded down to a power of two.  fp8: 0 = bf16, 1 = per-row fp8, 2 = MX fp8.  Returns 0, -3 (unknown bn) or -7 (MX
-// at bn 16).
+// at bn 16).  A bf16 / per-row fp8 decode launch (one token tile) that asks for the default depth may run a shallower
+// ring (>= 3 stages, same split-K) when that fits its whole grid in one wave; the output does not depend on the depth.
 int gemm_tc_resolve(int bn, int epi, int k, int fp8, int stages, int splitk, int* stages_out, int* splitk_out);
 int launch_gemm_tc(const GemmParams& p, const void* w, const void* x, int bn, cudaStream_t stream);
 

@@ -1,7 +1,11 @@
 """Per-CTA timeline of the GEMMs of consecutive decoder layers inside one CUDA graph (PDL chain, HBM-streamed
 weights): where do the kernel boundaries lose time?  Stamps (%globaltimer, 256 ns ticks): 0 CTA entry, 1 set-up done,
 2 producer: ring filled + producer released (pdl_wait / flag passed), 3 first MMA issued, 4 last MMA committed,
-5 accumulator visible to the epilogue warps, 6 epilogue stores done, 7 CTA exit."""
+5 accumulator visible to the epilogue warps, 6 epilogue stores done, 7 CTA exit.
+
+Per boundary between consecutive GEMMs it also prints the gap from the last exit of kernel n to the first MMA of kernel
+n+1, and how many of kernel n+1's CTAs had finished set-up and issued their weight prefetch (stamp 1) before that last
+exit: the weight stream that overlaps the boundary."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -44,7 +48,7 @@ first = log[3 * per_layer]
 t0 = int(h[first[4]: first[4] + first[5] * 8].view(-1, 8)[:, 0].min())
 print(f"B={B}; columns: min / median / max over the CTAs of a kernel, microseconds since layer 3 began")
 print(f"{'kernel':10s} {'ctas':>5s} | {'entry':>17s} | {'setup':>17s} | {'released':>17s} | {'1st mma':>17s} | {'last mma':>17s} | {'epi done':>17s} | {'exit':>17s}")
-prev_exit = None
+rows = []
 for (epi, n_out, k, sk, off, n) in log[3 * per_layer: 6 * per_layer]:
     v = (h[off: off + n * 8].view(n, 8).double() - t0) / 1e3
     def col(i):
@@ -52,4 +56,15 @@ for (epi, n_out, k, sk, off, n) in log[3 * per_layer: 6 * per_layer]:
         c = c[c > -1e6]
         return f"{c.min():5.1f} {c.median():5.1f} {c.max():5.1f}"
     nm = names.get(epi, "?") + (f"/{sk}" if sk > 1 else "")
+    rows.append((nm, v))
     print(f"{nm:10s} {n:5d} | {col(0)} | {col(1)} | {col(2)} | {col(3)} | {col(4)} | {col(6)} | {col(7)}")
+print()
+print("boundary             | last exit -> 1st mma (us) | CTAs of n+1 with prefetch issued before the last exit of n")
+for (na, va), (nb, vb) in zip(rows, rows[1:]):
+    def live(c):
+        return c[c > -1e6]
+    last_exit = live(va[:, 7]).max()
+    first_mma = live(vb[:, 3]).min()
+    setup = live(vb[:, 1])
+    early = int((setup < last_exit).sum())
+    print(f"{na:>9s} -> {nb:9s} | {first_mma - last_exit:25.2f} | {early:4d} / {len(setup)}")
