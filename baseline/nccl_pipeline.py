@@ -51,6 +51,8 @@ class NcclPipeline:
 
         self.cfg = c = resolve_config(model)
         assert c.norm == "rms" and c.glu, "comparator B covers the RMSNorm + GLU families (Llama / Mistral / Gemma-2)"
+        if c.rope_scaling:
+            raise ValueError(f"{c.name}: comparator B implements plain RoPE only, not rope_scaling {c.rope_scaling}")
         self.rank, self.world, self.dev = rank, world, device
         self.groups, self.gb, self.max_len = groups, group_batch, max_len
         self.first, self.last = rank == 0, rank == world - 1

@@ -528,7 +528,7 @@ class Engine:
             win = self._fetch_window(width, first=first)
         finished: List[int] = []
         now = time.time()
-        eos = self.cfg.eos_token_id
+        eos = list(self.cfg.eos_ids)
         if self.gpu:
             win = win.numpy()
         for b, r in list(self._running.items()):
@@ -547,7 +547,7 @@ class Engine:
             if not r.params.ignore_eos or r.params.stop_token_ids:
                 hit = np.zeros(take, dtype=bool)
                 if not r.params.ignore_eos:
-                    hit |= row[:take] == eos
+                    hit |= np.isin(row[:take], eos)
                 if r.params.stop_token_ids:
                     hit |= np.isin(row[:take], list(r.params.stop_token_ids))
                 nz = np.flatnonzero(hit)

@@ -12,7 +12,10 @@ import json
 import math
 import os
 from dataclasses import asdict, dataclass
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
+
+#: keys of a llama3 ``rope_scaling`` block (Llama-3.1 / 3.2 / 3.3), all required, as in transformers
+LLAMA3_ROPE_KEYS = ("factor", "low_freq_factor", "high_freq_factor", "original_max_position_embeddings")
 
 
 @dataclass
@@ -44,6 +47,10 @@ class ModelConfig:
     embed_scale: float = 1.0         # Gemma: sqrt(hidden)
     eos_token_id: int = -1
     bos_token_id: int = -1
+    # llama3 RoPE frequency transform: {"rope_type": "llama3", **LLAMA3_ROPE_KEYS}; None = plain RoPE.  The frequencies
+    # every layer uses come from ``rope_inv_freq``
+    rope_scaling: Optional[Dict] = None
+    eos_token_ids: Tuple[int, ...] = ()   # every EOS id of config.json (chat models list several); () = eos_token_id
 
     # ------------------------------------------------------------------ derived
     @property
@@ -53,6 +60,11 @@ class ModelConfig:
     @property
     def kv_dim(self) -> int:
         return self.n_kv_heads * self.head_dim
+
+    @property
+    def eos_ids(self) -> Tuple[int, ...]:
+        """ids that end a generation"""
+        return self.eos_token_ids or (self.eos_token_id,)
 
     @property
     def softmax_scale(self) -> float:
@@ -92,9 +104,19 @@ class ModelConfig:
         if d.get("attention_bias") or d.get("mlp_bias"):
             raise ValueError(f"{name or mt}: attention_bias / mlp_bias checkpoints (Qwen-style) are not supported: "
                              "the weight map carries no bias tensors for this family")
-        rs = d.get("rope_scaling")
-        if rs and (rs.get("rope_type") or rs.get("type") or "default") not in ("default",):
-            raise ValueError(f"{name or mt}: rope_scaling {rs!r} is not implemented (plain RoPE only)")
+        # legacy config.json: top-level rope_theta + rope_scaling; transformers >= 5 writes rope_parameters (theta inside)
+        rp = d.get("rope_parameters") or {}
+        rs = d.get("rope_scaling") or rp
+        kind = rs.get("rope_type") or rs.get("type") or "default"
+        if kind == "llama3":
+            scaling = _llama3_scaling(rs, name or mt)
+        elif kind == "default":
+            scaling = None
+        else:
+            raise ValueError(f"{name or mt}: rope_scaling {rs!r} is not implemented (plain RoPE and llama3 only)")
+        theta = d.get("rope_theta")
+        if theta is None:
+            theta = rp.get("rope_theta", 10000.0)
         h = d["hidden_size"]
         nh = d["num_attention_heads"]
         hd = d.get("head_dim") or h // nh
@@ -102,8 +124,9 @@ class ModelConfig:
             name=name or mt, vocab_size=d["vocab_size"], hidden_size=h, n_layers=d["num_hidden_layers"], n_heads=nh,
             n_kv_heads=d.get("num_key_value_heads", nh), head_dim=hd, ffn_size=d["intermediate_size"],
             max_position=d.get("max_position_embeddings", 8192), norm="rms", norm_eps=d.get("rms_norm_eps", 1e-5),
-            rope_theta=float(d.get("rope_theta", 10000.0)), tie_embeddings=bool(d.get("tie_word_embeddings", False)),
-            eos_token_id=_first_int(d.get("eos_token_id", -1)), bos_token_id=_first_int(d.get("bos_token_id", -1)))
+            rope_theta=float(theta), tie_embeddings=bool(d.get("tie_word_embeddings", False)),
+            eos_token_id=_first_int(d.get("eos_token_id", -1)), bos_token_id=_first_int(d.get("bos_token_id", -1)),
+            rope_scaling=scaling, eos_token_ids=_all_ints(d.get("eos_token_id")))
         if mt == "gemma2":
             return ModelConfig(
                 family="gemma2", act="gelu_tanh", glu=True, sliding_window=d.get("sliding_window", 4096),
@@ -131,8 +154,10 @@ class ModelConfig:
                 "intermediate_size": self.ffn_size, "max_position_embeddings": self.max_position,
                 "rms_norm_eps": self.norm_eps, "rope_theta": self.rope_theta,
                 "tie_word_embeddings": self.tie_embeddings, "bos_token_id": self.bos_token_id,
-                "eos_token_id": self.eos_token_id, "attention_bias": False, "mlp_bias": False,
-                "attention_dropout": 0.0}
+                "eos_token_id": list(self.eos_token_ids) if len(self.eos_token_ids) > 1 else self.eos_token_id,
+                "attention_bias": False, "mlp_bias": False, "attention_dropout": 0.0}
+        if self.rope_scaling:
+            base["rope_scaling"] = dict(self.rope_scaling)
         if self.family == "gemma2":
             base.update({"model_type": "gemma2", "architectures": ["Gemma2ForCausalLM"],
                          "hidden_activation": "gelu_pytorch_tanh", "sliding_window": self.sliding_window,
@@ -153,12 +178,63 @@ def _first_int(v) -> int:
     return -1 if v is None else int(v)
 
 
+def _all_ints(v) -> Tuple[int, ...]:
+    if isinstance(v, (list, tuple)):
+        return tuple(int(i) for i in v)
+    return () if v is None else (int(v),)
+
+
+def _llama3_scaling(rs: Dict, who: str) -> Dict:
+    """A validated llama3 block: all four LLAMA3_ROPE_KEYS present, factor >= 1, 0 < low_freq_factor < high_freq_factor."""
+    missing = [k for k in LLAMA3_ROPE_KEYS if rs.get(k) is None]
+    if missing:
+        raise ValueError(f"{who}: llama3 rope_scaling {rs!r} is missing {missing}")
+    out = {"rope_type": "llama3", "factor": float(rs["factor"]), "low_freq_factor": float(rs["low_freq_factor"]),
+           "high_freq_factor": float(rs["high_freq_factor"]),
+           "original_max_position_embeddings": int(rs["original_max_position_embeddings"])}
+    if not (out["factor"] >= 1.0 and 0.0 < out["low_freq_factor"] < out["high_freq_factor"]
+            and out["original_max_position_embeddings"] > 0):
+        raise ValueError(f"{who}: llama3 rope_scaling {rs!r} needs factor >= 1, 0 < low_freq_factor < "
+                         "high_freq_factor and original_max_position_embeddings > 0")
+    return out
+
+
+def rope_inv_freq(cfg: ModelConfig):
+    """The [head_dim/2] fp32 RoPE inverse frequencies of a llama3-scaled config, or None for plain RoPE (the kernels and
+    the oracle then compute theta^(-2j/head_dim) themselves).  Follows transformers' ``_compute_llama3_parameters``
+    operation for operation in fp32: pairs whose wavelength exceeds original_max_position_embeddings / low_freq_factor
+    turn ``factor`` times slower, pairs shorter than original / high_freq_factor keep their frequency, and the pairs in
+    between blend the two linearly in original / wavelength."""
+    rs = cfg.rope_scaling
+    if not rs:
+        return None
+    import torch
+
+    d = cfg.head_dim
+    inv = 1.0 / (cfg.rope_theta ** (torch.arange(0, d, 2, dtype=torch.int64).to(dtype=torch.float) / d))
+    factor, low, high = rs["factor"], rs["low_freq_factor"], rs["high_freq_factor"]
+    orig = rs["original_max_position_embeddings"]
+    wavelen = 2 * math.pi / inv
+    scaled = torch.where(wavelen > orig / low, inv / factor, inv)
+    smooth = (orig / wavelen - low) / (high - low)
+    smoothed = (1 - smooth) * scaled / factor + smooth * scaled
+    medium = ~(wavelen < orig / high) * ~(wavelen > orig / low)
+    return torch.where(medium, smoothed, scaled).contiguous()
+
+
 def _gpt2(name, layers, hidden, heads):
     return ModelConfig(name=name, family="gpt2", vocab_size=50257, hidden_size=hidden, n_layers=layers, n_heads=heads,
                        n_kv_heads=heads, head_dim=hidden // heads, ffn_size=4 * hidden, max_position=1024, norm="ln",
                        norm_eps=1e-5, act="gelu_tanh", glu=False, rope_theta=0.0, tie_embeddings=True, bias=True,
                        eos_token_id=50256, bos_token_id=50256)
 
+
+def _llama3(factor: float, original: int) -> Dict:
+    return {"rope_type": "llama3", "factor": factor, "low_freq_factor": 1.0, "high_freq_factor": 4.0,
+            "original_max_position_embeddings": original}
+
+
+_LLAMA3_EOS = (128001, 128008, 128009)
 
 PRESETS: Dict[str, ModelConfig] = {
     "distilgpt2": _gpt2("distilgpt2", 6, 768, 12),
@@ -194,6 +270,25 @@ PRESETS: Dict[str, ModelConfig] = {
     "mini-llama-4096": ModelConfig(name="mini-llama-4096", family="llama", vocab_size=32000, hidden_size=4096,
                                    n_layers=8, n_heads=32, n_kv_heads=8, head_dim=128, ffn_size=14336,
                                    rope_theta=500000.0, eos_token_id=1, bos_token_id=0),
+    # Llama-3.1 / 3.2: llama3-scaled RoPE over 128K positions.  The EOS tuple is the Instruct models' (<|end_of_text|>,
+    # <|eom_id|>, <|eot_id|>); the base models only emit the first.
+    "llama-3.1-8b": ModelConfig(name="llama-3.1-8b", family="llama", vocab_size=128256, hidden_size=4096, n_layers=32,
+                                n_heads=32, n_kv_heads=8, head_dim=128, ffn_size=14336, max_position=131072,
+                                norm_eps=1e-5, rope_theta=500000.0, eos_token_id=128001, bos_token_id=128000,
+                                rope_scaling=_llama3(8.0, 8192), eos_token_ids=_LLAMA3_EOS),
+    "llama-3.2-1b": ModelConfig(name="llama-3.2-1b", family="llama", vocab_size=128256, hidden_size=2048, n_layers=16,
+                                n_heads=32, n_kv_heads=8, head_dim=64, ffn_size=8192, max_position=131072,
+                                norm_eps=1e-5, rope_theta=500000.0, tie_embeddings=True, eos_token_id=128001,
+                                bos_token_id=128000, rope_scaling=_llama3(32.0, 8192), eos_token_ids=_LLAMA3_EOS),
+    "llama-3.2-3b": ModelConfig(name="llama-3.2-3b", family="llama", vocab_size=128256, hidden_size=3072, n_layers=28,
+                                n_heads=24, n_kv_heads=8, head_dim=128, ffn_size=8192, max_position=131072,
+                                norm_eps=1e-5, rope_theta=500000.0, tie_embeddings=True, eos_token_id=128001,
+                                bos_token_id=128000, rope_scaling=_llama3(32.0, 8192), eos_token_ids=_LLAMA3_EOS),
+    # tiny-llama with an original context of 64 positions: the scaling moves most rotary pairs within a few hundred
+    # tokens, so short test prompts see it
+    "tiny-llama31": ModelConfig(name="tiny-llama31", family="llama", vocab_size=512, hidden_size=256, n_layers=4,
+                                n_heads=4, n_kv_heads=2, head_dim=128, ffn_size=512, rope_theta=500000.0,
+                                eos_token_id=1, bos_token_id=0, rope_scaling=_llama3(8.0, 64)),
 }
 PRESETS["tiny-gpt2"].vocab_size = 384
 PRESETS["tiny-gpt2"].eos_token_id = 1
@@ -205,6 +300,13 @@ ALIASES = {
     "zephyr": "zephyr-7b-beta", "mistral-7b": "zephyr-7b-beta", "google/gemma-2-2b": "gemma-2-2b",
     "gemma2:2b": "gemma-2-2b", "gemma2": "gemma-2-2b", "distilbert/distilgpt2": "distilgpt2",
     "openai-community/gpt2": "gpt2",
+    "meta-llama/llama-3.1-8b": "llama-3.1-8b", "meta-llama/meta-llama-3.1-8b": "llama-3.1-8b",
+    "meta-llama/llama-3.1-8b-instruct": "llama-3.1-8b", "meta-llama/meta-llama-3.1-8b-instruct": "llama-3.1-8b",
+    "llama-3.1-8b-instruct": "llama-3.1-8b", "llama3.1": "llama-3.1-8b", "llama3.1:8b": "llama-3.1-8b",
+    "meta-llama/llama-3.2-1b": "llama-3.2-1b", "meta-llama/llama-3.2-1b-instruct": "llama-3.2-1b",
+    "llama-3.2-1b-instruct": "llama-3.2-1b", "llama3.2:1b": "llama-3.2-1b",
+    "meta-llama/llama-3.2-3b": "llama-3.2-3b", "meta-llama/llama-3.2-3b-instruct": "llama-3.2-3b",
+    "llama-3.2-3b-instruct": "llama-3.2-3b", "llama3.2": "llama-3.2-3b", "llama3.2:3b": "llama-3.2-3b",
 }
 
 

@@ -25,7 +25,7 @@ from typing import Dict, Iterable, Optional
 import torch
 
 from .. import ops
-from .config import ModelConfig
+from .config import ModelConfig, rope_inv_freq
 from .weights import Tensors
 
 
@@ -223,6 +223,9 @@ class NativePiece:
         if last:
             self.last_x = torch.zeros((max_seqs, H), device=dev, dtype=bf)
             self.logits = torch.zeros((max_seqs, self.vocab_pad), device=dev, dtype=torch.float32)
+        # scaled RoPE: the QKV epilogue reads its frequencies from this table (allocated once: graphs capture the address)
+        inv_freq = rope_inv_freq(c)
+        self.rope_freq = inv_freq.to(dev) if inv_freq is not None else None
         self.max_splits = 16
         g = c.n_heads // c.n_kv_heads
         rows = max(4, (g + 3) // 4 * 4)
@@ -372,7 +375,7 @@ class NativePiece:
                 qkv_kw = dict(epi=ops.EPI_QKV_ROPE, eps=eps, q_out=self.q_buf, k_cache=self.k_cache[l],
                               v_cache=self.v_cache[l], positions=m.positions, slots=m.slots, n_q_heads=c.n_heads,
                               n_kv_heads=c.n_kv_heads, head_dim=c.head_dim, rope_theta=c.rope_theta,
-                              q_scale=c.softmax_scale)
+                              rope_freq=self.rope_freq, q_scale=c.softmax_scale)
                 if self.fp8 and xq_ready:
                     # e4m3 copy + scale factors + sum of squares were produced by the previous layer's down epilogue
                     ops.gemm(self.w[p + "wqkv"], self._fq_x[:T], sfb=self._fq_sf_x, sumsq=self._sumsq1,

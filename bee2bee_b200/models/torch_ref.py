@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
-from .config import ModelConfig
+from .config import ModelConfig, rope_inv_freq
 from .weights import Tensors
 
 KV = Dict[int, Tuple[torch.Tensor, torch.Tensor]]
@@ -34,10 +34,14 @@ def gelu_tanh(x: torch.Tensor) -> torch.Tensor:
     return F.gelu(x, approximate="tanh")
 
 
-def rope(x: torch.Tensor, positions: torch.Tensor, theta: float) -> torch.Tensor:
-    """x [B, T, H, D]; rotate-half convention (pairs (i, i + D/2)), fp32 angles."""
+def rope(x: torch.Tensor, positions: torch.Tensor, theta: float, inv_freq: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """x [B, T, H, D]; rotate-half convention (pairs (i, i + D/2)), fp32 angles.  ``inv_freq``: the [D/2] frequency
+    table of a scaled config (``config.rope_inv_freq``); None = theta^(-2i/D)."""
     d = x.shape[-1]
-    inv = theta ** (-torch.arange(0, d, 2, device=x.device, dtype=torch.float32) / d)
+    if inv_freq is None:
+        inv = theta ** (-torch.arange(0, d, 2, device=x.device, dtype=torch.float32) / d)
+    else:
+        inv = inv_freq.to(x.device)
     ang = positions.float()[..., None] * inv                      # [B, T, D/2]
     cos, sin = ang.cos()[:, :, None, :], ang.sin()[:, :, None, :]
     x1, x2 = x.float()[..., : d // 2], x.float()[..., d // 2:]
@@ -49,6 +53,7 @@ class TorchPiece:
 
     def __init__(self, cfg: ModelConfig, layers: Iterable[int], first: bool, last: bool, tensors: Tensors):
         self.cfg, self.layers, self.first, self.last, self.t = cfg, list(layers), first, last, tensors
+        self.inv_freq = rope_inv_freq(cfg)
 
     # -- helpers -----------------------------------------------------------------
     def _norm(self, x, name: str):
@@ -87,7 +92,7 @@ class TorchPiece:
             k = self._lin(h, p + "wk", p + "bk").view(B, T, c.n_kv_heads, c.head_dim)
             v = self._lin(h, p + "wv", p + "bv").view(B, T, c.n_kv_heads, c.head_dim)
             if c.rope_theta > 0:
-                q, k = rope(q, positions, c.rope_theta), rope(k, positions, c.rope_theta)
+                q, k = rope(q, positions, c.rope_theta, self.inv_freq), rope(k, positions, c.rope_theta, self.inv_freq)
             k, v = k.transpose(1, 2), v.transpose(1, 2)                     # [B, n_kv, T, D]
             if cache is not None:
                 if l in cache:

@@ -193,8 +193,10 @@ def gemm(w: torch.Tensor, x: torch.Tensor, out: Optional[torch.Tensor] = None, *
          stages: int = -1, free_lag: int = 0, out2_ptr: int = 0,
          fq_out: Optional[torch.Tensor] = None, fq_sf: Optional[torch.Tensor] = None, fq_bn: int = 0,
          sumsq_out: Optional[torch.Tensor] = None, zero_buf: Optional[torch.Tensor] = None,
-         sumsq: Optional[torch.Tensor] = None, no_out: bool = False) -> Optional[torch.Tensor]:
-    """out[t, n] = epilogue(sum_k x[t, k] * w[n, k]) on the wgmma swap-AB kernel."""
+         sumsq: Optional[torch.Tensor] = None, no_out: bool = False,
+         rope_freq: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+    """out[t, n] = epilogue(sum_k x[t, k] * w[n, k]) on the wgmma swap-AB kernel.  ``rope_freq``: EPI_QKV_ROPE with
+    scaled RoPE, the [head_dim/2] fp32 inverse frequencies (``models.config.rope_inv_freq``) on the GEMM's device."""
     m_tok, k = x.shape
     n_out = w.shape[0]
     if bn <= 0:
@@ -238,7 +240,7 @@ def gemm(w: torch.Tensor, x: torch.Tensor, out: Optional[torch.Tensor] = None, *
                   q_scale, wait_flag, wait_epoch, signal_flag, signal_epoch, done_counter, free_flag, bump_epoch,
                   ack_flag, dbg, w_scale, sfa, sfb, stages, free_lag, out2_ptr,
                   _ptr(fq_out), _ptr(fq_sf), fq_out.shape[1] if fq_out is not None else 0, fq_bn, _ptr(sumsq_out), _ptr(zero_buf),
-                  _ptr(sumsq))
+                  _ptr(sumsq), rope_freq)
     return out
 
 

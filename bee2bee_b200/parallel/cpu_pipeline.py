@@ -149,7 +149,7 @@ class MeshPipelineService(BaseService):
                 seen.add(tok)
                 if on_token is not None:
                     on_token(tok)
-                if tok == self.cfg.eos_token_id or step == max_new - 1:
+                if tok in self.cfg.eos_ids or step == max_new - 1:
                     break
                 p = len(prompt_ids) + step
                 logits = await self._through_chain(session, torch.tensor([[tok]]), [p], reset=False)

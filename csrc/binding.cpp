@@ -48,7 +48,9 @@ void gemm(const Tensor& w, const Tensor& x, int64_t out_ptr, int64_t ld_out, int
           int64_t free_flag, int64_t bump_epoch, int64_t ack_flag, int64_t dbg, const OptT& w_scale,
           const OptT& sfa, const OptT& sfb, int64_t stages, int64_t free_lag, int64_t out2_ptr,
           // fused MX quantisation of the output / RMSNorm statistics (raw addresses, 0 = off)
-          int64_t q_out8, int64_t q_sf, int64_t ld_q, int64_t q_bn, int64_t sumsq_out, int64_t zero_buf, int64_t sumsq) {
+          int64_t q_out8, int64_t q_sf, int64_t ld_q, int64_t q_bn, int64_t sumsq_out, int64_t zero_buf, int64_t sumsq,
+          // scaled RoPE: [head_dim/2] fp32 inverse frequencies, or none
+          const OptT& rope_freq) {
   const bool fp8 = w.scalar_type() == at::kFloat8_e4m3fn;
   if (fp8) {
     TORCH_CHECK(x.scalar_type() == at::kFloat8_e4m3fn && w.is_cuda() && x.is_cuda() && w.is_contiguous() &&
@@ -112,6 +114,7 @@ void gemm(const Tensor& w, const Tensor& x, int64_t out_ptr, int64_t ld_out, int
   p.n_kv_heads = static_cast<int16_t>(n_kv_heads);
   p.head_dim = static_cast<int16_t>(head_dim);
   p.rope_theta = static_cast<float>(rope_theta);
+  p.rope_freq = ptr_or_null<const float>(rope_freq);
   p.q_scale = static_cast<float>(q_scale);
   p.wait_flag = as_ptr<const uint32_t>(wait_flag);
   p.wait_epoch = as_ptr<const uint32_t>(wait_epoch);
@@ -126,6 +129,13 @@ void gemm(const Tensor& w, const Tensor& x, int64_t out_ptr, int64_t ld_out, int
   if (p.epi == b2b::EPI_QKV_ROPE) {
     TORCH_CHECK(p.q_out && p.k_cache && p.v_cache && p.slots, "qkv epilogue needs q_out/k_cache/v_cache/slots");
     TORCH_CHECK(p.rope_theta <= 0.f || p.positions, "rope needs positions");
+    if (rope_freq.has_value()) {
+      TORCH_CHECK(rope_freq->is_cuda() && rope_freq->scalar_type() == at::kFloat && rope_freq->is_contiguous() &&
+                      rope_freq->numel() == head_dim / 2 && rope_freq->device() == w.device(),
+                  "rope_freq must be a contiguous fp32 tensor of head_dim/2 = ", head_dim / 2,
+                  " entries on the GEMM's device");
+      TORCH_CHECK(p.rope_theta > 0.f, "rope_freq needs rope_theta > 0");
+    }
     TORCH_CHECK((p.n_q_heads * p.head_dim) % 128 == 0 && (p.n_kv_heads * p.head_dim) % 128 == 0,
                 "q/kv widths must be multiples of 128");
     TORCH_CHECK(p.n_out == (p.n_q_heads + 2 * p.n_kv_heads) * p.head_dim, "qkv rows mismatch");

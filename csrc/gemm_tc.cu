@@ -425,7 +425,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       f_in_sect = f - (sect == 0 ? 0 : (sect == 1 ? q_dim : q_dim + kv_dim));
       if (sect < 2 && p.rope_theta > 0.f) {
         const int j = (f_in_sect % p.head_dim) >> 1;   // rotary pair index (rows are pair-interleaved)
-        inv_freq = exp2f(-(2.f * j / static_cast<float>(p.head_dim)) * log2f(p.rope_theta));
+        inv_freq = p.rope_freq ? p.rope_freq[j]
+                               : exp2f(-(2.f * j / static_cast<float>(p.head_dim)) * log2f(p.rope_theta));
       }
     }
 

@@ -66,6 +66,7 @@ struct GemmParams {
   const int* slots;               // [m_tok] physical KV slot of each token
   int16_t n_q_heads, n_kv_heads, head_dim;
   float rope_theta;               // <=0: no rotary
+  const float* rope_freq;         // [head_dim/2] inverse frequency per rotary pair (scaled RoPE), or null = theta^(-2j/hd)
   float q_scale;                  // folded softmax scale applied to q (1.0 = none)
 
   // NVLink piece handoff ---------------------------------------------------
