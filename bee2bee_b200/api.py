@@ -106,6 +106,8 @@ class ChatRequest(BaseModel):
     stream: Optional[bool] = False
     top_k: Optional[int] = None       # keep the k most likely tokens; absent = off
     min_p: Optional[float] = None     # keep tokens with p >= min_p * p_max; absent = off
+    presence_penalty: Optional[float] = None    # in [-2, 2], subtracted from every generated token; absent = off
+    frequency_penalty: Optional[float] = None   # in [-2, 2], times each generated token's count; absent = off
 
 
 @app.get("/")
@@ -208,7 +210,8 @@ async def chat(req: ChatRequest):
         return {"status": "error", "message": "node not started"}
     params = {"prompt": req.prompt, "max_new_tokens": req.max_new_tokens or 2048,
               "temperature": 0.7 if req.temperature is None else req.temperature}
-    filters = sampling_filters({"top_k": req.top_k, "min_p": req.min_p})
+    filters = sampling_filters({"top_k": req.top_k, "min_p": req.min_p, "presence_penalty": req.presence_penalty,
+                                "frequency_penalty": req.frequency_penalty})
     params.update(filters)
     try:
         t0 = time.time()

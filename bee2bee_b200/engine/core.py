@@ -26,7 +26,7 @@ import numpy as np
 import torch
 
 from ..models.config import ModelConfig, resolve_config, split_layers
-from ..models.torch_ref import TorchPiece, sample_reference
+from ..models.torch_ref import COUNT_MAX, TorchPiece, sample_reference
 from ..models.weights import load_or_init
 from .kv import PAGE, PageAllocator
 
@@ -39,6 +39,8 @@ class SamplingParams:
     repetition_penalty: float = 1.15   # reference streaming default (hf.py:95)
     top_k: int = 0                     # keep the k most likely tokens (ties kept) before top-p; 0 = off
     min_p: float = 0.0                 # after top-p keep tokens with p >= min_p * p_max; 0 = off
+    presence_penalty: float = 0.0      # subtracted from every token generated so far (prompt excluded); 0 = off
+    frequency_penalty: float = 0.0     # times the token's generated count, subtracted too; 0 = off
     seed: Optional[int] = None
     stop_token_ids: Sequence[int] = ()
     ignore_eos: bool = False
@@ -109,9 +111,18 @@ class TorchRunner:
         V = self.cfg.vocab_size
         seen = torch.zeros(1, V, dtype=torch.bool)
         seen[0, torch.tensor(sorted(st["seen"]), dtype=torch.long)] = True
+        counts = None
+        if st["presence"] != 0.0 or st["frequency"] != 0.0:
+            counts = torch.zeros(1, V, dtype=torch.int32)
+            if st["counts"]:
+                ids = list(st["counts"])
+                counts[0, torch.tensor(ids, dtype=torch.long)] = torch.tensor([st["counts"][i] for i in ids],
+                                                                              dtype=torch.int32)
         tok = int(sample_reference(logits[None, :V].cpu(), seen, st["temperature"], st["top_p"], st["rep"],
-                                   st["gen"], top_k=st["top_k"], min_p=st["min_p"]))
+                                   st["gen"], top_k=st["top_k"], min_p=st["min_p"], counts=counts,
+                                   presence=st["presence"], frequency=st["frequency"]))
         st["seen"].add(tok)
+        st["counts"][tok] = min(st["counts"].get(tok, 0) + 1, COUNT_MAX)
         return tok
 
     def prefill(self, seqs) -> None:
@@ -120,8 +131,8 @@ class TorchRunner:
                 self.cache.pop(s.slot, None)
                 g = torch.Generator().manual_seed(int(s.seed) & 0x7FFFFFFF)
                 st = dict(temperature=s.temperature, top_p=s.top_p, rep=s.repetition_penalty, top_k=s.top_k,
-                          min_p=s.min_p, gen=g,
-                          seen=set(int(t) for t in s.prompt), pos=len(s.prompt), hist=[])
+                          min_p=s.min_p, presence=s.presence_penalty, frequency=s.frequency_penalty, gen=g,
+                          seen=set(int(t) for t in s.prompt), counts={}, pos=len(s.prompt), hist=[])
                 logits = self._forward(s.slot, list(s.prompt), 0)
                 tok = self._sample(st, logits)
                 st["hist"].append(tok)
@@ -230,6 +241,10 @@ class Engine:
             raise ValueError(f"top_k must be >= 0 (0 = off), got {params.top_k}")
         if not 0.0 <= params.min_p <= 1.0:
             raise ValueError(f"min_p must lie in [0, 1] (0 = off), got {params.min_p}")
+        for name in ("presence_penalty", "frequency_penalty"):
+            v = getattr(params, name)
+            if not -2.0 <= v <= 2.0:          # also refuses NaN and +-inf
+                raise ValueError(f"{name} must be a finite value in [-2, 2] (0 = off), got {v}")
         ids = list(prompt_ids)[-(self.max_seq_len - 1):] or [max(self.cfg.bos_token_id, 0)]
         budget = self.max_seq_len - len(ids)
         if params.max_new_tokens > budget:
@@ -423,7 +438,8 @@ class Engine:
                             repetition_penalty=r.params.repetition_penalty,
                             # k >= vocab already means off; the clamp keeps any k a client sends inside int32
                             top_k=min(int(r.params.top_k), self.cfg.vocab_size),
-                            min_p=r.params.min_p, seed=r.params.seed if r.params.seed is not None else (r.rid * 2654435761) & 0x7FFFFFFF,
+                            min_p=r.params.min_p, presence_penalty=r.params.presence_penalty,
+                            frequency_penalty=r.params.frequency_penalty, seed=r.params.seed if r.params.seed is not None else (r.rid * 2654435761) & 0x7FFFFFFF,
                             cached=self.alloc.cached_tokens(r.slot))
                     for r in admitted]
             for r in admitted:          # after the whole admission round: requests of one round never share with each other

@@ -45,6 +45,8 @@ class SeqInit:
     repetition_penalty: float = 1.15
     top_k: int = 0           # 0 = off
     min_p: float = 0.0       # 0 = off
+    presence_penalty: float = 0.0    # 0 = off
+    frequency_penalty: float = 0.0   # 0 = off
     seed: int = 0
     cached: int = 0          # leading prompt tokens whose KV is already resident in ``pages`` (prefix cache): not prefilled
 
@@ -143,11 +145,15 @@ class GpuRunner:
         self.top_p = torch.ones(B, device=dev)
         self.top_k = torch.zeros(B, device=dev, dtype=i32)
         self.min_p = torch.zeros(B, device=dev)
+        self.presence = torch.zeros(B, device=dev)
+        self.frequency = torch.zeros(B, device=dev)
         self.rep_pen = torch.ones(B, device=dev)
         self.seeds = torch.zeros(B, device=dev, dtype=i32)
         self.hist_pos = torch.zeros(B, device=dev, dtype=i32)
         self.step_ctr = torch.zeros(1, device=dev, dtype=i32)
         self.seen = torch.zeros((B, (cfg.vocab_size + 31) // 32), device=dev, dtype=i32)
+        # times each id was generated per slot (presence / frequency penalties); read and written by the sampler only
+        self.counts = ops.counts_table(B, cfg.vocab_size, dev) if self.last else None
         self.tok_local = torch.zeros(B, device=dev, dtype=i32)     # last rank's own copy of sampled ids
         self.graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self._pf: Dict[tuple, dict] = {}           # prefill state (staging + graph) per bucket
@@ -246,8 +252,8 @@ class GpuRunner:
         for i, s in enumerate(seqs):
             bt_np[i, :len(s.pages)] = s.pages
         bt_host = torch.from_numpy(bt_np)
-        fl_host = torch.tensor([[s.temperature, s.top_p, s.repetition_penalty, s.min_p] for s in seqs],
-                               dtype=torch.float32)
+        fl_host = torch.tensor([[s.temperature, s.top_p, s.repetition_penalty, s.min_p, s.presence_penalty,
+                                 s.frequency_penalty] for s in seqs], dtype=torch.float32)
         # seed and top_k in one int32 copy
         int_host = torch.tensor([[int(s.seed) & 0x7FFFFFFF, int(s.top_k)] for s in seqs], dtype=i32)
         rows = torch.tensor([s.slot for s in seqs], dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
@@ -258,10 +264,14 @@ class GpuRunner:
         self.top_p.index_copy_(0, rows, fl[:, 1].contiguous())
         self.rep_pen.index_copy_(0, rows, fl[:, 2].contiguous())
         self.min_p.index_copy_(0, rows, fl[:, 3].contiguous())
+        self.presence.index_copy_(0, rows, fl[:, 4].contiguous())
+        self.frequency.index_copy_(0, rows, fl[:, 5].contiguous())
         self.seeds.index_copy_(0, rows, iv[:, 0].contiguous())
         self.top_k.index_copy_(0, rows, iv[:, 1].contiguous())
         self.hist_pos.index_fill_(0, rows, 0)
         self.seen.index_fill_(0, rows, 0)
+        if self.counts is not None:
+            self.counts.index_fill_(0, rows, 0)
         self.h2d_bytes += bt_host.numel() * 4 + fl_host.numel() * 4 + int_host.numel() * 4 + S * 8
         if self.last:
             flat = np.concatenate([np.asarray(s.prompt, dtype=np.int32) for s in seqs])
@@ -343,8 +353,8 @@ class GpuRunner:
                 multi = self.world > 1
                 ops.sample(out, self.tok_local if multi else self.tokens, seen=self.seen, temperature=self.temperature,
                            top_p=self.top_p, top_k=self.top_k, min_p=self.min_p, rep_penalty=self.rep_pen,
-                           seeds=self.seeds, step=self.step_ctr,
-                           vocab=self.cfg.vocab_size, softcap=self.cfg.final_softcap,
+                           seeds=self.seeds, step=self.step_ctr, counts=self.counts, presence=self.presence,
+                           frequency=self.frequency, vocab=self.cfg.vocab_size, softcap=self.cfg.final_softcap,
                            history=self.mesh.hist_base() if multi else self.history.data_ptr(), hist_pos=self.hist_pos,
                            hist_stride=self.hist_len, peer_tokens=self.mesh.tok_base() if multi else 0,
                            row_map=v["row_map"].data_ptr())
@@ -441,6 +451,8 @@ class GpuRunner:
                        seen=self._grp(self.seen, g), temperature=self._grp(self.temperature, g),
                        top_p=self._grp(self.top_p, g), top_k=self._grp(self.top_k, g),
                        min_p=self._grp(self.min_p, g), rep_penalty=self._grp(self.rep_pen, g),
+                       counts=self._grp(self.counts, g), presence=self._grp(self.presence, g),
+                       frequency=self._grp(self.frequency, g),
                        seeds=self._grp(self.seeds, g), step=self.step_ctr, vocab=self.cfg.vocab_size,
                        softcap=self.cfg.final_softcap, history=hist_ptr, hist_pos=self._grp(self.hist_pos, g),
                        hist_stride=self.hist_len, peer_tokens=hand.out_x if multi else 0,
@@ -493,6 +505,8 @@ class GpuRunner:
         self.hist_pos.zero_()
         self.step_ctr.zero_()
         self.seen.zero_()
+        if self.counts is not None:
+            self.counts.zero_()         # the warm-up decode published into every row
         self.tokens.zero_()
         torch.cuda.synchronize(self.device)
 

@@ -140,18 +140,28 @@ class TorchPiece:
         return logits
 
 
+COUNT_MAX = 32767       # generated-token counts saturate here (the sampler's int16 count table)
+
+
 def sample_reference(logits: torch.Tensor, seen: Optional[torch.Tensor], temperature: float, top_p: float,
                      rep_penalty: float, generator: Optional[torch.Generator] = None, top_k: int = 0,
-                     min_p: float = 0.0) -> torch.Tensor:
-    """HF-processor semantics (repetition penalty -> temperature -> top-k -> top-p -> min-p -> multinomial /
-    greedy when temperature <= 0), cf. /root/reference/bee2bee/hf.py:91-105.
+                     min_p: float = 0.0, counts: Optional[torch.Tensor] = None, presence: float = 0.0,
+                     frequency: float = 0.0) -> torch.Tensor:
+    """HF-processor semantics (repetition penalty -> presence / frequency penalty -> temperature -> top-k -> top-p ->
+    min-p -> multinomial / greedy when temperature <= 0), cf. /root/reference/bee2bee/hf.py:91-105.
     logits [B, V] fp32; seen [B, V] bool of ids already in the context.  ``top_k`` keeps the tokens at least as likely
     as the k-th (ties kept; <= 0 or >= V = off); top-p then sees the top-k survivors renormalised; ``min_p`` keeps
-    p >= min_p * p_max (<= 0 = off)."""
+    p >= min_p * p_max (<= 0 = off).  ``counts`` [B, V] holds how often each id was generated (prompt excluded); where
+    it is positive, l = (l - frequency * c) - presence in fp32, as vLLM / OpenAI define the two penalties (0 = off);
+    greedy rows are penalised too."""
     l = logits.float().clone()
     if seen is not None and rep_penalty != 1.0:
         pen = torch.where(l > 0, l / rep_penalty, l * rep_penalty)
         l = torch.where(seen, pen, l)
+    if counts is not None and (presence != 0.0 or frequency != 0.0):
+        c = counts.to(torch.float32)
+        pf = (l - torch.tensor(frequency, dtype=torch.float32) * c) - torch.tensor(presence, dtype=torch.float32)
+        l = torch.where(counts > 0, pf, l)
     if not temperature > 0:
         return l.argmax(-1)
     l = l / temperature

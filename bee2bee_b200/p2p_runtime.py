@@ -675,9 +675,12 @@ class P2PNode:
                                  model_name: Optional[str] = None, temperature: float = 0.7, stream: bool = False,
                                  on_chunk: Optional[Callable[[str], None]] = None,
                                  timeout: float = DEFAULT_GEN_TIMEOUT, top_k: Optional[int] = None,
-                                 min_p: Optional[float] = None) -> Dict[str, Any]:
-        """``top_k`` / ``min_p``: optional sampling filters (None = off), passed on only when set."""
-        filters = sampling_filters({"top_k": top_k, "min_p": min_p})
+                                 min_p: Optional[float] = None, presence_penalty: Optional[float] = None,
+                                 frequency_penalty: Optional[float] = None) -> Dict[str, Any]:
+        """``top_k`` / ``min_p`` / ``presence_penalty`` / ``frequency_penalty``: optional sampling controls (None =
+        off), passed on only when set."""
+        filters = sampling_filters({"top_k": top_k, "min_p": min_p, "presence_penalty": presence_penalty,
+                                    "frequency_penalty": frequency_penalty})
         params = {"prompt": prompt, "max_new_tokens": max_new_tokens, "temperature": temperature, **filters}
         if provider_id == self.peer_id:
             svc = self._find_local_service(None, model_name)

@@ -25,7 +25,7 @@ import torch
 
 from ..engine.tokenizer import STOP_WORDS, cut_at_stop_words, load_tokenizer, parse_transcript
 from ..models.config import ModelConfig, resolve_config, split_layers
-from ..models.torch_ref import TorchPiece, sample_reference
+from ..models.torch_ref import COUNT_MAX, TorchPiece, sample_reference
 from ..models.weights import load_or_init
 from ..services import BaseService, ServiceError, sampling_filters
 from ..utils import new_id
@@ -130,10 +130,13 @@ class MeshPipelineService(BaseService):
 
     async def agenerate(self, prompt_ids: List[int], max_new: int, temperature: float, top_p: float = 1.0,
                         rep: float = 1.0, on_token=None, seed: int = 0, top_k: int = 0,
-                        min_p: float = 0.0) -> List[int]:
+                        min_p: float = 0.0, presence_penalty: float = 0.0,
+                        frequency_penalty: float = 0.0) -> List[int]:
         session = new_id("sess")
         gen = torch.Generator().manual_seed(seed)
         seen = set(prompt_ids)
+        penalised = presence_penalty != 0.0 or frequency_penalty != 0.0
+        counts = torch.zeros(1, self.cfg.vocab_size, dtype=torch.int32)     # generated tokens only
         out: List[int] = []
         V = self.cfg.vocab_size
         try:
@@ -144,9 +147,11 @@ class MeshPipelineService(BaseService):
                 seen_mask = torch.zeros(1, V, dtype=torch.bool)
                 seen_mask[0, torch.tensor(sorted(seen), dtype=torch.long)] = True
                 tok = int(sample_reference(logits[0, -1:, :V], seen_mask, temperature, top_p, rep, gen, top_k=top_k,
-                                           min_p=min_p))
+                                           min_p=min_p, counts=counts if penalised else None,
+                                           presence=presence_penalty, frequency=frequency_penalty))
                 out.append(tok)
                 seen.add(tok)
+                counts[0, tok] = min(int(counts[0, tok]) + 1, COUNT_MAX)
                 if on_token is not None:
                     on_token(tok)
                 if tok in self.cfg.eos_ids or step == max_new - 1:

@@ -77,7 +77,8 @@ def service_announce(service: str, meta: Dict[str, Any]) -> Dict[str, Any]:
 
 def gen_request(rid: str, prompt: str, model: Optional[str] = None, svc: str = "hf", max_new_tokens: int = 2048,
                 temperature: float = 0.7, stream: bool = False, top_k: Optional[int] = None,
-                min_p: Optional[float] = None) -> Dict[str, Any]:
+                min_p: Optional[float] = None, presence_penalty: Optional[float] = None,
+                frequency_penalty: Optional[float] = None) -> Dict[str, Any]:
     # both spellings are sent: the reference reads ``max_tokens`` but its requester writes
     # ``max_new_tokens`` (p2p_runtime.py:577 vs 822)
     m = msg(GEN_REQUEST, rid=rid, prompt=prompt, model=model, svc=svc, max_new_tokens=max_new_tokens,
@@ -87,6 +88,10 @@ def gen_request(rid: str, prompt: str, model: Optional[str] = None, svc: str = "
         m["top_k"] = int(top_k)
     if min_p is not None:
         m["min_p"] = float(min_p)
+    if presence_penalty is not None:
+        m["presence_penalty"] = float(presence_penalty)
+    if frequency_penalty is not None:
+        m["frequency_penalty"] = float(frequency_penalty)
     return m
 
 

@@ -34,12 +34,14 @@ class ServiceError(Exception):
 
 
 def sampling_filters(params: Dict[str, Any]) -> Dict[str, Any]:
-    """The ``top_k`` / ``min_p`` a request sets (absent or null = off), as keyword arguments."""
+    """The ``top_k`` / ``min_p`` / ``presence_penalty`` / ``frequency_penalty`` a request sets (absent or null = off),
+    as keyword arguments."""
     out: Dict[str, Any] = {}
     if params.get("top_k") is not None:
         out["top_k"] = int(params["top_k"])
-    if params.get("min_p") is not None:
-        out["min_p"] = float(params["min_p"])
+    for name in ("min_p", "presence_penalty", "frequency_penalty"):
+        if params.get(name) is not None:
+            out[name] = float(params[name])
     return out
 
 
@@ -202,8 +204,10 @@ class EmbeddedOllama:
         lm = self._ensure()
         opts = payload.get("options") or {}
         # top_k / min_p only when the request sets them: Ollama's own top_k default (40) is not applied.  Ollama (like
-        # llama.cpp) treats top_k <= 0 and min_p <= 0 as off, so negative values mean off here too.
-        filters = {k: v if v > 0 else type(v)(0) for k, v in sampling_filters(opts).items()}
+        # llama.cpp) treats top_k <= 0 and min_p <= 0 as off, so negative values mean off here too.  presence_penalty /
+        # frequency_penalty likewise only when present; negative values favour repetition, as in Ollama.
+        filters = {k: (v if v > 0 else type(v)(0)) if k in ("top_k", "min_p") else v
+                   for k, v in sampling_filters(opts).items()}
         sp = SamplingParams(max_new_tokens=int(opts.get("num_predict", 128)),
                             temperature=float(opts.get("temperature", 0.8)), top_p=float(opts.get("top_p", 0.9)),
                             repetition_penalty=float(opts.get("repeat_penalty", 1.1)), **filters)

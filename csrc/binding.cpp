@@ -387,7 +387,8 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
             int64_t history, const OptT& hist_pos, int64_t hist_stride, int64_t vocab, double softcap,
             const OptT& temperature, const OptT& top_p,
             const OptT& rep_penalty, const OptT& seeds, const OptT& step, int64_t signal_flag, int64_t signal_epoch,
-            int64_t done_counter, int64_t row_map, const OptT& top_k, const OptT& min_p) {
+            int64_t done_counter, int64_t row_map, const OptT& top_k, const OptT& min_p, const OptT& counts,
+            const OptT& presence, const OptT& frequency) {
   TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.stride(1) == 1, "logits: fp32");
   // top_k / min_p are per-sequence state like temperature: one entry per state row (logits row b reads row
   // row_map[b], or b without a row_map)
@@ -403,6 +404,22 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
   };
   check_row_param(top_k, at::kInt, "top_k");
   check_row_param(min_p, at::kFloat, "min_p");
+  check_row_param(presence, at::kFloat, "presence");
+  check_row_param(frequency, at::kFloat, "frequency");
+  const int64_t V = vocab > 0 ? vocab : logits.size(1);
+  const bool has_counts = counts.has_value() && counts->defined();
+  if (has_counts) {
+    // [state rows, cstride] int16, rows padded to a multiple of 8 ids so that 4 ids are one aligned 8-byte load
+    const Tensor& c = *counts;
+    TORCH_CHECK(c.scalar_type() == at::kShort && c.device() == logits.device() && c.dim() == 2 && c.stride(1) == 1,
+                "counts must be a 2-D int16 tensor with unit column stride on the logits' device");
+    TORCH_CHECK(c.size(0) == state_rows && (row_map != 0 || c.size(0) >= logits.size(0)), "counts has ", c.size(0),
+                " rows; expected one per state row (", state_rows, ")");
+    TORCH_CHECK(c.size(1) >= V && c.stride(0) >= V && c.stride(0) % 8 == 0 &&
+                    (reinterpret_cast<uintptr_t>(c.data_ptr()) & 7) == 0,
+                "counts rows must hold the vocabulary (", V, " ids) at a row stride that is a multiple of 8 ids, "
+                "from an 8-byte aligned address; got ", c.size(1), " ids at stride ", c.stride(0));
+  }
   c10::cuda::CUDAGuard guard(logits.device());
   int* hp = ptr_or_null<int>(hist_pos);
   check(b2b::launch_sample(reinterpret_cast<const float*>(logits.data_ptr()), ptr_or_null<uint32_t>(seen),
@@ -414,7 +431,9 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
                            ptr_or_null<const float>(rep_penalty), ptr_or_null<const uint32_t>(seeds),
                            ptr_or_null<const uint32_t>(step), as_ptr<uint32_t>(signal_flag),
                            as_ptr<uint32_t>(signal_epoch), as_ptr<uint32_t>(done_counter), as_ptr<const int>(row_map),
-                           ptr_or_null<const int>(top_k), ptr_or_null<const float>(min_p), cur_stream()),
+                           ptr_or_null<const int>(top_k), ptr_or_null<const float>(min_p), ptr_or_null<int16_t>(counts),
+                           has_counts ? static_cast<int>(counts->stride(0)) : 0, ptr_or_null<const float>(presence),
+                           ptr_or_null<const float>(frequency), cur_stream()),
         "sample");
 }
 

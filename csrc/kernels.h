@@ -49,7 +49,8 @@ int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* pee
                   const int* hist_pos, int* hist_pos_out, int hist_stride, int batch, int vocab, int ld, float softcap,
                   const float* temperature, const float* top_p, const float* rep_penalty, const uint32_t* seeds,
                   const uint32_t* step, uint32_t* signal_flag, uint32_t* signal_epoch, uint32_t* done_counter,
-                  const int* row_map, const int* top_k, const float* min_p, cudaStream_t s);
+                  const int* row_map, const int* top_k, const float* min_p, int16_t* counts, int counts_stride,
+                  const float* presence, const float* frequency, cudaStream_t s);
 // CTAs per sequence (1, 2, 4 or 8) that launch_sample runs a batch at on a device with `sms` SMs; 0 = the vocabulary
 // does not fit in shared memory at any cluster size
 int sample_cluster_size(int batch, int vocab, int sms);

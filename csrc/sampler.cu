@@ -1,5 +1,5 @@
-// Fused sampler for sm_90a: repetition penalty (seen-token bitmap) -> temperature -> top-k ->
-// top-p -> min-p, each decided on a two-level radix histogram of the probability bits ->
+// Fused sampler for sm_90a: repetition penalty (seen-token bitmap) -> presence / frequency
+// penalty (per-row counts of generated tokens) -> temperature -> top-k -> top-p -> min-p, each decided on a two-level radix histogram of the probability bits ->
 // multinomial draw (or argmax when temperature <= 0).  One cluster per sequence, logits are
 // fp32 [B, ld] as written by the lm_head GEMM.  The sampled id is stored locally (token ring,
 // history bitmap) and, on the last piece of a pipeline, straight into piece 0's token buffer on
@@ -7,6 +7,13 @@
 //
 // Semantics follow the reference's generation defaults (bee2bee/hf.py:91-105):
 // repetition_penalty 1.15, top_p 0.95, do_sample iff temperature > 0, greedy otherwise.
+// Presence / frequency penalties (vLLM / OpenAI; per row, 0 = off) run after the repetition penalty:
+// with c the number of times the id has been generated for the row (prompt excluded; an int16
+// table that saturates at 32767), l = (l - f c) - p when c > 0, in explicit round-to-nearest steps
+// (no FMA contraction, so an fp32 reference reproduces it bit for bit).  A row reads its counts only
+// when p or f is non-zero (row-uniform branch; a row with both off runs the unchanged phase-1 loop),
+// greedy rows included.  When a count table is given, the publishing thread increments the drawn
+// id's count (saturating); every CTA of the cluster has read its counts before the draw.
 // After temperature the filters run in transformers' processor order, with e = exp(l - max):
 //   * top-k (k per row; k <= 0 or k >= V = off): K = the tokens whose e is at least the k-th
 //     largest e, ties at the k-th value kept.  K is decided on the same 22-bit key (top 22 bits
@@ -58,6 +65,10 @@ struct SampleParams {
   const int* top_k;         // [rows] (<= 0 or >= vocab = off), or null
   const float* min_p;       // [rows] (<= 0 = off), or null
   const float* rep_penalty; // [rows]
+  int16_t* counts;          // [rows, cstride] times each id was generated (saturates at 32767), or null
+  int cstride;              // row stride of counts in ids (a multiple of 8)
+  const float* presence;    // [rows] presence penalty p (0 = off), or null
+  const float* frequency;   // [rows] frequency penalty f (0 = off), or null
   const uint32_t* seeds;    // [rows]
   const uint32_t* step;     // device step counter (rng stream), may be null
   uint32_t* signal_flag;    // peer flag (token handoff) or null
@@ -70,6 +81,15 @@ struct SampleParams {
 __device__ __forceinline__ float transform(float l, bool is_seen, float pen, float inv_temp, float cap) {
   if (cap > 0.f) l = cap * tanhf(l / cap);
   if (is_seen) l = l > 0.f ? l / pen : l * pen;
+  return l * inv_temp;
+}
+
+// transform() with the presence / frequency penalty between the repetition penalty and temperature
+__device__ __forceinline__ float transform_pf(float l, bool is_seen, int c, float pen, float pres, float freq,
+                                             float inv_temp, float cap) {
+  if (cap > 0.f) l = cap * tanhf(l / cap);
+  if (is_seen) l = l > 0.f ? l / pen : l * pen;
+  if (c > 0) l = __fsub_rn(__fsub_rn(l, __fmul_rn(freq, static_cast<float>(c))), pres);
   return l * inv_temp;
 }
 
@@ -168,11 +188,20 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
   const uint32_t* seen_r = (pen != 1.f) ? seen : nullptr;
   const int lo = min(V, r * W), hi = min(V, lo + W), n = hi - lo;
   const int n4 = n >> 2;
+  const float pres = p.presence ? p.presence[bb] : 0.f;
+  const float freq = p.frequency ? p.frequency[bb] : 0.f;
+  const int16_t* cnt = (p.counts != nullptr && (pres != 0.f || freq != 0.f))
+                           ? p.counts + static_cast<size_t>(bb) * p.cstride : nullptr;
 
   // exactly one thread per sequence publishes the token
   auto publish = [&](int token) {
     p.out_tokens[bb] = token;
     if (seen != nullptr) atomicOr(&seen[token >> 5], 1u << (token & 31));
+    if (p.counts != nullptr) {
+      int16_t* c = p.counts + static_cast<size_t>(bb) * p.cstride + token;
+      const int16_t v = *c;
+      if (v < 32767) *c = static_cast<int16_t>(v + 1);
+    }
     if (p.history != nullptr) {
       const int pos = p.hist_pos[bb];
       // the history is a ring: the host reads each burst's window before the writer can lap it
@@ -185,7 +214,33 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
 
   // ---- phase 1: L2 -> (soft-cap, penalty, temperature) -> shared memory; running max / argmax
   float mx = -INFINITY; int amx = 0;
-  {
+  if (cnt != nullptr) {
+    // penalised row: 4 ids per iteration, their counts in one aligned 8-byte load
+    auto take = [&](int i, float raw, uint32_t sw, int c) {
+      const float l = transform_pf(raw, (sw >> (i & 31)) & 1u, c, pen, pres, freq, inv_temp, cap);
+      ebuf[i - lo] = l;
+      if (l > mx) { mx = l; amx = i; }
+    };
+    for (int q = tid; q < n4; q += SAMP_THREADS) {
+      const int i0 = lo + 4 * q;
+      float a[4];
+      if (vec_ok) {
+        const float4 va = *reinterpret_cast<const float4*>(logits + i0);
+        a[0] = va.x; a[1] = va.y; a[2] = va.z; a[3] = va.w;
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) a[k] = logits[i0 + k];
+      }
+      const uint2 cw = *reinterpret_cast<const uint2*>(cnt + i0);
+      const uint32_t sa = seen_r ? seen_r[i0 >> 5] : 0u;
+      take(i0, a[0], sa, static_cast<int16_t>(cw.x & 0xFFFFu));
+      take(i0 + 1, a[1], sa, static_cast<int16_t>(cw.x >> 16));
+      take(i0 + 2, a[2], sa, static_cast<int16_t>(cw.y & 0xFFFFu));
+      take(i0 + 3, a[3], sa, static_cast<int16_t>(cw.y >> 16));
+    }
+    for (int i = lo + 4 * n4 + tid; i < hi; i += SAMP_THREADS)
+      take(i, logits[i], seen_r ? seen_r[i >> 5] : 0u, cnt[i]);
+  } else {
     auto take = [&](int i, float raw, uint32_t sw) {
       const float l = transform(raw, (sw >> (i & 31)) & 1u, pen, inv_temp, cap);
       ebuf[i - lo] = l;
@@ -526,11 +581,16 @@ int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* pee
                   const int* hist_pos, int* hist_pos_out, int hist_stride, int batch, int vocab, int ld, float softcap,
                   const float* temperature, const float* top_p, const float* rep_penalty, const uint32_t* seeds,
                   const uint32_t* step, uint32_t* signal_flag, uint32_t* signal_epoch, uint32_t* done_counter,
-                  const int* row_map, const int* top_k, const float* min_p, cudaStream_t s) {
+                  const int* row_map, const int* top_k, const float* min_p, int16_t* counts, int counts_stride,
+                  const float* presence, const float* frequency, cudaStream_t s) {
+  if (counts != nullptr && (counts_stride < vocab || counts_stride % 8 != 0 ||
+                            (reinterpret_cast<uintptr_t>(counts) & 7) != 0))
+    return -7;
   SampleParams p;
   p.logits = logits; p.seen = seen; p.out_tokens = out_tokens; p.peer_tokens = peer_tokens; p.history = history;
   p.hist_pos = hist_pos; p.hist_pos_out = hist_pos_out; p.hist_stride = hist_stride; p.vocab = vocab; p.ld = ld; p.softcap = softcap;
   p.temperature = temperature; p.top_p = top_p; p.top_k = top_k; p.min_p = min_p; p.rep_penalty = rep_penalty;
+  p.counts = counts; p.cstride = counts_stride; p.presence = presence; p.frequency = frequency;
   p.seeds = seeds; p.step = step;
   p.signal_flag = signal_flag; p.signal_epoch = signal_epoch; p.done_counter = done_counter; p.row_map = row_map;
   if (sample_cluster_size(1, vocab, 0) == 0) return -6;

@@ -1,6 +1,8 @@
-"""Time ``sample`` at B=32, V=128256 (Llama-3 vocabulary), T=0.7, repetition penalty 1.15, for four filter settings:
-off (top_p 0.95), top_k=50, top_k=50 with top_p=0.95, and min_p=0.05.  The settings run in one process and alternate
-round by round, so clock and neighbour load drift hit all of them alike.  Prints the card and its power limit."""
+"""Time ``sample`` at B=32, V=128256 (Llama-3 vocabulary), T=0.7, repetition penalty 1.15, for these settings:
+off (top_p 0.95), top_k=50, top_k=50 with top_p=0.95, min_p=0.05; off with a count table (what the engine runs when a
+request sets no penalty: the table is only written); presence and frequency penalties 0.5 over a count table with a
+few hundred distinct ids per row, alone and with top_k=50.  The settings run in one process and alternate round by
+round, so clock and neighbour load drift hit all of them alike.  Prints the card and its power limit."""
 import os
 import subprocess
 import sys
@@ -28,6 +30,12 @@ t = torch.full((B,), 0.7, device=dev)
 rp = torch.full((B,), 1.15, device=dev)
 seeds = torch.arange(B, device=dev, dtype=torch.int32)
 step = torch.zeros(1, device=dev, dtype=torch.int32)
+# a generation history: 400 distinct ids per row, each generated 1 to 12 times
+counts = ops.counts_table(B, V, dev)
+gen = torch.Generator(device="cpu").manual_seed(1)
+for b in range(B):
+    ids = torch.randperm(V, generator=gen)[:400]
+    counts[b, ids.to(dev)] = torch.randint(1, 13, (400,), generator=gen, dtype=torch.int16).to(dev)
 
 
 def full(v, dtype=torch.float32):
@@ -39,6 +47,10 @@ rows = {
     "top_k=50": dict(top_p=full(1.0), top_k=full(50, torch.int32), min_p=full(0.0)),
     "top_k=50 top_p=0.95": dict(top_p=full(0.95), top_k=full(50, torch.int32), min_p=full(0.0)),
     "min_p=0.05": dict(top_p=full(1.0), top_k=full(0, torch.int32), min_p=full(0.05)),
+    "off + count table": dict(top_p=full(0.95), counts=counts, presence=full(0.0), frequency=full(0.0)),
+    "p=0.5 f=0.5": dict(top_p=full(0.95), counts=counts, presence=full(0.5), frequency=full(0.5)),
+    "p=0.5 f=0.5 top_k=50": dict(top_p=full(0.95), top_k=full(50, torch.int32), min_p=full(0.0), counts=counts,
+                                 presence=full(0.5), frequency=full(0.5)),
 }
 
 
@@ -62,5 +74,5 @@ for _ in range(ROUNDS):
         times[name].append(e0.elapsed_time(e1) * 1e3 / ITERS)
 for name, ts in times.items():
     ts = sorted(ts)
-    print(f"sampler B={B} V={V} {name:22s}: median {ts[len(ts) // 2]:.1f} us  (min {ts[0]:.1f}, max {ts[-1]:.1f}, "
+    print(f"sampler B={B} V={V} {name:24s}: median {ts[len(ts) // 2]:.1f} us  (min {ts[0]:.1f}, max {ts[-1]:.1f}, "
           f"{ROUNDS} rounds x {ITERS} launches)")
