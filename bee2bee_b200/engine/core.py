@@ -19,21 +19,22 @@ import queue
 import statistics
 import threading
 import time
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, fields
 from typing import Callable, Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
 
 from ..models.config import ModelConfig, resolve_config, split_layers
-from ..models.torch_ref import COUNT_MAX, TorchPiece, sample_reference
+from ..models.torch_ref import SequenceSampler, TorchPiece
 from ..models.weights import load_or_init
 from .kv import PAGE, PageAllocator
 
 
-@dataclass
-class SamplingParams:
-    max_new_tokens: int = 32
+@dataclass(kw_only=True)
+class SamplerControls:
+    """A sequence's sampling controls: the request carries them (``SamplingParams``), the replicated plan hands them
+    to every rank (``runner.SeqInit``), and the sampler applies them per sequence."""
     temperature: float = 0.7
     top_p: float = 0.95                # reference streaming default (hf.py:103)
     repetition_penalty: float = 1.15   # reference streaming default (hf.py:95)
@@ -41,6 +42,26 @@ class SamplingParams:
     min_p: float = 0.0                 # after top-p keep tokens with p >= min_p * p_max; 0 = off
     presence_penalty: float = 0.0      # subtracted from every token generated so far (prompt excluded); 0 = off
     frequency_penalty: float = 0.0     # times the token's generated count, subtracted too; 0 = off
+
+    def validate(self) -> None:
+        """Raise ``ValueError`` for a control outside the range the sampler defines."""
+        if not self.top_k >= 0:
+            raise ValueError(f"top_k must be >= 0 (0 = off), got {self.top_k}")
+        if not 0.0 <= self.min_p <= 1.0:
+            raise ValueError(f"min_p must lie in [0, 1] (0 = off), got {self.min_p}")
+        for name in ("presence_penalty", "frequency_penalty"):
+            v = getattr(self, name)
+            if not -2.0 <= v <= 2.0:          # also refuses NaN and +-inf
+                raise ValueError(f"{name} must be a finite value in [-2, 2] (0 = off), got {v}")
+
+    def controls(self) -> Dict[str, object]:
+        """The controls alone, as keyword arguments for another ``SamplerControls``."""
+        return {f.name: getattr(self, f.name) for f in fields(SamplerControls)}
+
+
+@dataclass(kw_only=True)
+class SamplingParams(SamplerControls):
+    max_new_tokens: int = 32
     seed: Optional[int] = None
     stop_token_ids: Sequence[int] = ()
     ignore_eos: bool = False
@@ -107,36 +128,14 @@ class TorchRunner:
                 x = self.hop(i, x)
         return x[0, -1]
 
-    def _sample(self, st: dict, logits: torch.Tensor) -> int:
-        V = self.cfg.vocab_size
-        seen = torch.zeros(1, V, dtype=torch.bool)
-        seen[0, torch.tensor(sorted(st["seen"]), dtype=torch.long)] = True
-        counts = None
-        if st["presence"] != 0.0 or st["frequency"] != 0.0:
-            counts = torch.zeros(1, V, dtype=torch.int32)
-            if st["counts"]:
-                ids = list(st["counts"])
-                counts[0, torch.tensor(ids, dtype=torch.long)] = torch.tensor([st["counts"][i] for i in ids],
-                                                                              dtype=torch.int32)
-        tok = int(sample_reference(logits[None, :V].cpu(), seen, st["temperature"], st["top_p"], st["rep"],
-                                   st["gen"], top_k=st["top_k"], min_p=st["min_p"], counts=counts,
-                                   presence=st["presence"], frequency=st["frequency"]))
-        st["seen"].add(tok)
-        st["counts"][tok] = min(st["counts"].get(tok, 0) + 1, COUNT_MAX)
-        return tok
-
     def prefill(self, seqs) -> None:
         with torch.no_grad():
             for s in seqs:
                 self.cache.pop(s.slot, None)
-                g = torch.Generator().manual_seed(int(s.seed) & 0x7FFFFFFF)
-                st = dict(temperature=s.temperature, top_p=s.top_p, rep=s.repetition_penalty, top_k=s.top_k,
-                          min_p=s.min_p, presence=s.presence_penalty, frequency=s.frequency_penalty, gen=g,
-                          seen=set(int(t) for t in s.prompt), counts={}, pos=len(s.prompt), hist=[])
-                logits = self._forward(s.slot, list(s.prompt), 0)
-                tok = self._sample(st, logits)
-                st["hist"].append(tok)
-                self.state[s.slot] = st
+                sampler = SequenceSampler(s, self.cfg.vocab_size, s.prompt,
+                                          torch.Generator().manual_seed(int(s.seed) & 0x7FFFFFFF))
+                tok = sampler.draw(self._forward(s.slot, list(s.prompt), 0))
+                self.state[s.slot] = dict(sampler=sampler, pos=len(s.prompt), hist=[tok])
 
     def decode(self, n_steps: int) -> None:
         with torch.no_grad():
@@ -146,7 +145,7 @@ class TorchRunner:
                         continue
                     logits = self._forward(slot, [st["hist"][-1]], st["pos"])
                     st["pos"] += 1
-                    st["hist"].append(self._sample(st, logits))
+                    st["hist"].append(st["sampler"].draw(logits))
 
     def sync(self) -> None:
         pass
@@ -237,14 +236,7 @@ class Engine:
     def submit(self, prompt_ids: Sequence[int], params: Optional[SamplingParams] = None,
                on_token: Optional[Callable[[int], None]] = None) -> Request:
         params = params or SamplingParams()
-        if not params.top_k >= 0:
-            raise ValueError(f"top_k must be >= 0 (0 = off), got {params.top_k}")
-        if not 0.0 <= params.min_p <= 1.0:
-            raise ValueError(f"min_p must lie in [0, 1] (0 = off), got {params.min_p}")
-        for name in ("presence_penalty", "frequency_penalty"):
-            v = getattr(params, name)
-            if not -2.0 <= v <= 2.0:          # also refuses NaN and +-inf
-                raise ValueError(f"{name} must be a finite value in [-2, 2] (0 = off), got {v}")
+        params.validate()
         ids = list(prompt_ids)[-(self.max_seq_len - 1):] or [max(self.cfg.bos_token_id, 0)]
         budget = self.max_seq_len - len(ids)
         if params.max_new_tokens > budget:
@@ -434,12 +426,9 @@ class Engine:
         self._pending = still
         if admitted:
             seqs = [SeqInit(slot=r.slot, prompt=r.prompt_ids, pages=self.alloc.owned(r.slot),
-                            temperature=r.params.temperature, top_p=r.params.top_p,
-                            repetition_penalty=r.params.repetition_penalty,
                             # k >= vocab already means off; the clamp keeps any k a client sends inside int32
-                            top_k=min(int(r.params.top_k), self.cfg.vocab_size),
-                            min_p=r.params.min_p, presence_penalty=r.params.presence_penalty,
-                            frequency_penalty=r.params.frequency_penalty, seed=r.params.seed if r.params.seed is not None else (r.rid * 2654435761) & 0x7FFFFFFF,
+                            **{**r.params.controls(), "top_k": min(int(r.params.top_k), self.cfg.vocab_size)},
+                            seed=r.params.seed if r.params.seed is not None else (r.rid * 2654435761) & 0x7FFFFFFF,
                             cached=self.alloc.cached_tokens(r.slot))
                     for r in admitted]
             for r in admitted:          # after the whole admission round: requests of one round never share with each other

@@ -31,24 +31,25 @@ from ..models.config import UNITS_PER_LAYER, ModelConfig, piece_units, unit_laye
 from ..models.native import BatchMeta, NativePiece
 from ..models.weights import load_or_init
 from ..parallel.mesh import F_TOK_DONE, MeshComm
+from .core import SamplerControls
 from .kv import PAGE
 
 
-@dataclass
-class SeqInit:
+@dataclass(kw_only=True)
+class SeqInit(SamplerControls):
     """Everything a rank needs to start a sequence (part of the replicated plan)."""
     slot: int
     prompt: List[int]
     pages: List[int]
-    temperature: float = 0.7
-    top_p: float = 0.95
-    repetition_penalty: float = 1.15
-    top_k: int = 0           # 0 = off
-    min_p: float = 0.0       # 0 = off
-    presence_penalty: float = 0.0    # 0 = off
-    frequency_penalty: float = 0.0   # 0 = off
     seed: int = 0
     cached: int = 0          # leading prompt tokens whose KV is already resident in ``pages`` (prefix cache): not prefilled
+
+
+# The sampler's per-slot rows on the device, as (SeqInit field, ``ops.sample`` keyword) in the row order of the fp32
+# block and of the int32 block.  Every field is a contiguous row, and so is any slot range of it.
+SAMPLER_F32_ROWS = (("temperature", "temperature"), ("top_p", "top_p"), ("repetition_penalty", "rep_penalty"),
+                    ("min_p", "min_p"), ("presence_penalty", "presence"), ("frequency_penalty", "frequency"))
+SAMPLER_I32_ROWS = (("seed", "seeds"), ("top_k", "top_k"))
 
 
 def _pow2_at_least(n: int, lo: int = 1) -> int:
@@ -141,14 +142,11 @@ class GpuRunner:
         self.slots = torch.full((B,), -1, device=dev, dtype=i32)
         self.block_table = torch.zeros((B, self.max_pages_per_seq), device=dev, dtype=i32)
         self.q_start = torch.arange(self.gb, device=dev, dtype=i32)
-        self.temperature = torch.zeros(B, device=dev)
-        self.top_p = torch.ones(B, device=dev)
-        self.top_k = torch.zeros(B, device=dev, dtype=i32)
-        self.min_p = torch.zeros(B, device=dev)
-        self.presence = torch.zeros(B, device=dev)
-        self.frequency = torch.zeros(B, device=dev)
-        self.rep_pen = torch.ones(B, device=dev)
-        self.seeds = torch.zeros(B, device=dev, dtype=i32)
+        # sampler controls per slot; a slot that holds no sequence samples greedily with every filter and penalty off
+        idle = SamplerControls(temperature=0.0, top_p=1.0, repetition_penalty=1.0)
+        self.sampler_f32 = torch.tensor([[getattr(idle, f)] * B for f, _ in SAMPLER_F32_ROWS], device=dev,
+                                        dtype=torch.float32)
+        self.sampler_i32 = torch.zeros((len(SAMPLER_I32_ROWS), B), device=dev, dtype=i32)    # seed 0, top_k 0 = off
         self.hist_pos = torch.zeros(B, device=dev, dtype=i32)
         self.step_ctr = torch.zeros(1, device=dev, dtype=i32)
         self.seen = torch.zeros((B, (cfg.vocab_size + 31) // 32), device=dev, dtype=i32)
@@ -192,6 +190,23 @@ class GpuRunner:
     # ------------------------------------------------------------------ helpers
     def _grp(self, t: torch.Tensor, g: int) -> torch.Tensor:
         return t[g * self.gb:(g + 1) * self.gb]
+
+    def _sampler_rows(self, lo: int, hi: int) -> dict:
+        """``ops.sample`` keyword arguments of the per-slot state of slots [lo, hi)."""
+        kw = {k: self.sampler_f32[r, lo:hi] for r, (_, k) in enumerate(SAMPLER_F32_ROWS)}
+        kw.update({k: self.sampler_i32[r, lo:hi] for r, (_, k) in enumerate(SAMPLER_I32_ROWS)})
+        return dict(kw, seen=self.seen[lo:hi], counts=self.counts[lo:hi], hist_pos=self.hist_pos[lo:hi])
+
+    def _reset_sampler_state(self, rows: Optional[torch.Tensor] = None) -> None:
+        """Clear what the sampler accumulates per slot (history write position, seen bitmap, generated-token counts)
+        for the slots ``rows`` (int64 on the device), or for every slot."""
+        for t in (self.hist_pos, self.seen, self.counts):
+            if t is None:
+                continue                    # the count table lives on the last piece only
+            if rows is None:
+                t.zero_()
+            else:
+                t.index_fill_(0, rows, 0)
 
     def launches_per_decode_step(self) -> int:
         """Native kernel launches one rank issues per group decode step: counted while the decode graph was recorded
@@ -252,26 +267,15 @@ class GpuRunner:
         for i, s in enumerate(seqs):
             bt_np[i, :len(s.pages)] = s.pages
         bt_host = torch.from_numpy(bt_np)
-        fl_host = torch.tensor([[s.temperature, s.top_p, s.repetition_penalty, s.min_p, s.presence_penalty,
-                                 s.frequency_penalty] for s in seqs], dtype=torch.float32)
-        # seed and top_k in one int32 copy
-        int_host = torch.tensor([[int(s.seed) & 0x7FFFFFFF, int(s.top_k)] for s in seqs], dtype=i32)
+        fl_host = torch.tensor([[getattr(s, f) for s in seqs] for f, _ in SAMPLER_F32_ROWS], dtype=torch.float32)
+        # the seed keeps its low 31 bits
+        int_host = torch.tensor([[int(getattr(s, f)) & 0x7FFFFFFF if f == "seed" else int(getattr(s, f)) for s in seqs]
+                                 for f, _ in SAMPLER_I32_ROWS], dtype=i32)
         rows = torch.tensor([s.slot for s in seqs], dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
-        fl = fl_host.pin_memory().to(dev, non_blocking=True)
-        iv = int_host.pin_memory().to(dev, non_blocking=True)
         self.block_table.index_copy_(0, rows, bt_host.pin_memory().to(dev, non_blocking=True))
-        self.temperature.index_copy_(0, rows, fl[:, 0].contiguous())
-        self.top_p.index_copy_(0, rows, fl[:, 1].contiguous())
-        self.rep_pen.index_copy_(0, rows, fl[:, 2].contiguous())
-        self.min_p.index_copy_(0, rows, fl[:, 3].contiguous())
-        self.presence.index_copy_(0, rows, fl[:, 4].contiguous())
-        self.frequency.index_copy_(0, rows, fl[:, 5].contiguous())
-        self.seeds.index_copy_(0, rows, iv[:, 0].contiguous())
-        self.top_k.index_copy_(0, rows, iv[:, 1].contiguous())
-        self.hist_pos.index_fill_(0, rows, 0)
-        self.seen.index_fill_(0, rows, 0)
-        if self.counts is not None:
-            self.counts.index_fill_(0, rows, 0)
+        self.sampler_f32.index_copy_(1, rows, fl_host.pin_memory().to(dev, non_blocking=True))
+        self.sampler_i32.index_copy_(1, rows, int_host.pin_memory().to(dev, non_blocking=True))
+        self._reset_sampler_state(rows)
         self.h2d_bytes += bt_host.numel() * 4 + fl_host.numel() * 4 + int_host.numel() * 4 + S * 8
         if self.last:
             flat = np.concatenate([np.asarray(s.prompt, dtype=np.int32) for s in seqs])
@@ -351,11 +355,9 @@ class GpuRunner:
             out = self.piece.forward(meta, x_in=x_in, hand=hand, h_in=h_in)
             if self.last:
                 multi = self.world > 1
-                ops.sample(out, self.tok_local if multi else self.tokens, seen=self.seen, temperature=self.temperature,
-                           top_p=self.top_p, top_k=self.top_k, min_p=self.min_p, rep_penalty=self.rep_pen,
-                           seeds=self.seeds, step=self.step_ctr, counts=self.counts, presence=self.presence,
-                           frequency=self.frequency, vocab=self.cfg.vocab_size, softcap=self.cfg.final_softcap,
-                           history=self.mesh.hist_base() if multi else self.history.data_ptr(), hist_pos=self.hist_pos,
+                ops.sample(out, self.tok_local if multi else self.tokens, **self._sampler_rows(0, self.max_batch),
+                           step=self.step_ctr, vocab=self.cfg.vocab_size, softcap=self.cfg.final_softcap,
+                           history=self.mesh.hist_base() if multi else self.history.data_ptr(),
                            hist_stride=self.hist_len, peer_tokens=self.mesh.tok_base() if multi else 0,
                            row_map=v["row_map"].data_ptr())
                 if multi:
@@ -448,13 +450,8 @@ class GpuRunner:
             multi = self.world > 1
             hist_ptr = (self.mesh.history_ptr(g) if multi else self._grp(self.history, g).data_ptr())
             ops.sample(out, self._grp(self.tok_local, g) if multi else self._grp(self.tokens, g),
-                       seen=self._grp(self.seen, g), temperature=self._grp(self.temperature, g),
-                       top_p=self._grp(self.top_p, g), top_k=self._grp(self.top_k, g),
-                       min_p=self._grp(self.min_p, g), rep_penalty=self._grp(self.rep_pen, g),
-                       counts=self._grp(self.counts, g), presence=self._grp(self.presence, g),
-                       frequency=self._grp(self.frequency, g),
-                       seeds=self._grp(self.seeds, g), step=self.step_ctr, vocab=self.cfg.vocab_size,
-                       softcap=self.cfg.final_softcap, history=hist_ptr, hist_pos=self._grp(self.hist_pos, g),
+                       **self._sampler_rows(g * gb, (g + 1) * gb), step=self.step_ctr, vocab=self.cfg.vocab_size,
+                       softcap=self.cfg.final_softcap, history=hist_ptr,
                        hist_stride=self.hist_len, peer_tokens=hand.out_x if multi else 0,
                        signal_flag=hand.out_flag if multi else 0, signal_epoch=hand.out_epoch if multi else 0,
                        done_counter=(self.mesh._flag(self.mesh.local, g, F_TOK_DONE) if multi else 0))
@@ -502,11 +499,8 @@ class GpuRunner:
         self.q_len.copy_(saved)
         self.positions.copy_(pos)
         self.kv_len.copy_(kvl)
-        self.hist_pos.zero_()
+        self._reset_sampler_state()     # the warm-up decode sampled into every row
         self.step_ctr.zero_()
-        self.seen.zero_()
-        if self.counts is not None:
-            self.counts.zero_()         # the warm-up decode published into every row
         self.tokens.zero_()
         torch.cuda.synchronize(self.device)
 

@@ -180,6 +180,29 @@ def sample_reference(logits: torch.Tensor, seen: Optional[torch.Tensor], tempera
     return torch.multinomial(l.softmax(-1), 1, generator=generator).squeeze(-1)
 
 
+class SequenceSampler:
+    """One sequence's sampling on the CPU: its controls (any ``engine.core.SamplerControls``), its generator, the ids
+    in its context (repetition penalty) and how often each id was generated (presence / frequency penalties)."""
+
+    def __init__(self, controls, vocab: int, prompt: Iterable[int], generator: torch.Generator):
+        self.controls, self.generator = controls, generator
+        self.seen = torch.zeros(1, vocab, dtype=torch.bool)
+        self.seen[0, torch.tensor(sorted({int(t) for t in prompt}), dtype=torch.long)] = True
+        self.counts = torch.zeros(1, vocab, dtype=torch.int32)       # generated tokens only, saturating at COUNT_MAX
+
+    def draw(self, logits: torch.Tensor) -> int:
+        """The next id from ``logits`` [>= vocab] of the sequence's last position; it is then seen and counted."""
+        c = self.controls
+        penalised = c.presence_penalty != 0.0 or c.frequency_penalty != 0.0
+        tok = int(sample_reference(logits[None, :self.seen.shape[1]].cpu(), self.seen, c.temperature, c.top_p,
+                                   c.repetition_penalty, self.generator, top_k=c.top_k, min_p=c.min_p,
+                                   counts=self.counts if penalised else None, presence=c.presence_penalty,
+                                   frequency=c.frequency_penalty))
+        self.seen[0, tok] = True
+        self.counts[0, tok] = min(int(self.counts[0, tok]) + 1, COUNT_MAX)
+        return tok
+
+
 def top_p_keep_mask(logits: torch.Tensor, temperature: float, top_p: float) -> torch.Tensor:
     """[B, V] bool: the nucleus the sampler is allowed to draw from (oracle for the CUDA sampler)."""
     l = logits.float() / temperature

@@ -23,9 +23,10 @@ from typing import Any, Dict, Iterator, List, Optional
 
 import torch
 
+from ..engine.core import SamplerControls
 from ..engine.tokenizer import STOP_WORDS, cut_at_stop_words, load_tokenizer, parse_transcript
 from ..models.config import ModelConfig, resolve_config, split_layers
-from ..models.torch_ref import COUNT_MAX, TorchPiece, sample_reference
+from ..models.torch_ref import SequenceSampler, TorchPiece
 from ..models.weights import load_or_init
 from ..services import BaseService, ServiceError, sampling_filters
 from ..utils import new_id
@@ -133,25 +134,17 @@ class MeshPipelineService(BaseService):
                         min_p: float = 0.0, presence_penalty: float = 0.0,
                         frequency_penalty: float = 0.0) -> List[int]:
         session = new_id("sess")
-        gen = torch.Generator().manual_seed(seed)
-        seen = set(prompt_ids)
-        penalised = presence_penalty != 0.0 or frequency_penalty != 0.0
-        counts = torch.zeros(1, self.cfg.vocab_size, dtype=torch.int32)     # generated tokens only
+        controls = SamplerControls(temperature=temperature, top_p=top_p, repetition_penalty=rep, top_k=top_k,
+                                   min_p=min_p, presence_penalty=presence_penalty, frequency_penalty=frequency_penalty)
+        sampler = SequenceSampler(controls, self.cfg.vocab_size, prompt_ids, torch.Generator().manual_seed(seed))
         out: List[int] = []
-        V = self.cfg.vocab_size
         try:
             x = torch.tensor([prompt_ids])
             pos = list(range(len(prompt_ids)))
             logits = await self._through_chain(session, x, pos, reset=True)
             for step in range(max_new):
-                seen_mask = torch.zeros(1, V, dtype=torch.bool)
-                seen_mask[0, torch.tensor(sorted(seen), dtype=torch.long)] = True
-                tok = int(sample_reference(logits[0, -1:, :V], seen_mask, temperature, top_p, rep, gen, top_k=top_k,
-                                           min_p=min_p, counts=counts if penalised else None,
-                                           presence=presence_penalty, frequency=frequency_penalty))
+                tok = sampler.draw(logits[0, -1])
                 out.append(tok)
-                seen.add(tok)
-                counts[0, tok] = min(int(counts[0, tok]) + 1, COUNT_MAX)
                 if on_token is not None:
                     on_token(tok)
                 if tok in self.cfg.eos_ids or step == max_new - 1:

@@ -421,20 +421,33 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
                 "from an 8-byte aligned address; got ", c.size(1), " ids at stride ", c.stride(0));
   }
   c10::cuda::CUDAGuard guard(logits.device());
-  int* hp = ptr_or_null<int>(hist_pos);
-  check(b2b::launch_sample(reinterpret_cast<const float*>(logits.data_ptr()), ptr_or_null<uint32_t>(seen),
-                           reinterpret_cast<int*>(out_tokens.data_ptr()), as_ptr<int>(peer_tokens),
-                           as_ptr<int>(history), hp, hp, static_cast<int>(hist_stride),
-                           static_cast<int>(logits.size(0)), static_cast<int>(vocab > 0 ? vocab : logits.size(1)),
-                           static_cast<int>(logits.stride(0)), static_cast<float>(softcap),
-                           ptr_or_null<const float>(temperature), ptr_or_null<const float>(top_p),
-                           ptr_or_null<const float>(rep_penalty), ptr_or_null<const uint32_t>(seeds),
-                           ptr_or_null<const uint32_t>(step), as_ptr<uint32_t>(signal_flag),
-                           as_ptr<uint32_t>(signal_epoch), as_ptr<uint32_t>(done_counter), as_ptr<const int>(row_map),
-                           ptr_or_null<const int>(top_k), ptr_or_null<const float>(min_p), ptr_or_null<int16_t>(counts),
-                           has_counts ? static_cast<int>(counts->stride(0)) : 0, ptr_or_null<const float>(presence),
-                           ptr_or_null<const float>(frequency), cur_stream()),
-        "sample");
+  b2b::SampleParams p{};
+  p.logits = reinterpret_cast<const float*>(logits.data_ptr());
+  p.seen = ptr_or_null<uint32_t>(seen);
+  p.out_tokens = reinterpret_cast<int*>(out_tokens.data_ptr());
+  p.peer_tokens = as_ptr<int>(peer_tokens);
+  p.history = as_ptr<int>(history);
+  p.hist_pos = p.hist_pos_out = ptr_or_null<int>(hist_pos);
+  p.hist_stride = static_cast<int>(hist_stride);
+  p.vocab = static_cast<int>(V);
+  p.ld = static_cast<int>(logits.stride(0));
+  p.softcap = static_cast<float>(softcap);
+  p.temperature = ptr_or_null<const float>(temperature);
+  p.top_p = ptr_or_null<const float>(top_p);
+  p.top_k = ptr_or_null<const int>(top_k);
+  p.min_p = ptr_or_null<const float>(min_p);
+  p.rep_penalty = ptr_or_null<const float>(rep_penalty);
+  p.counts = ptr_or_null<int16_t>(counts);
+  p.cstride = has_counts ? static_cast<int>(counts->stride(0)) : 0;
+  p.presence = ptr_or_null<const float>(presence);
+  p.frequency = ptr_or_null<const float>(frequency);
+  p.seeds = ptr_or_null<const uint32_t>(seeds);
+  p.step = ptr_or_null<const uint32_t>(step);
+  p.signal_flag = as_ptr<uint32_t>(signal_flag);
+  p.signal_epoch = as_ptr<uint32_t>(signal_epoch);
+  p.done_counter = as_ptr<uint32_t>(done_counter);
+  p.row_map = as_ptr<const int>(row_map);
+  check(b2b::launch_sample(p, static_cast<int>(logits.size(0)), cur_stream()), "sample");
 }
 
 // CTAs per sequence that `sample` runs a batch of `batch` rows at on the current device (0 = vocabulary too large)

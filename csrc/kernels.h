@@ -45,12 +45,36 @@ int launch_attention_merge(void* out, const int* q_start, const int* q_len, cons
 int attention_init();
 
 // sampler.cu
-int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* peer_tokens, int* history,
-                  const int* hist_pos, int* hist_pos_out, int hist_stride, int batch, int vocab, int ld, float softcap,
-                  const float* temperature, const float* top_p, const float* rep_penalty, const uint32_t* seeds,
-                  const uint32_t* step, uint32_t* signal_flag, uint32_t* signal_epoch, uint32_t* done_counter,
-                  const int* row_map, const int* top_k, const float* min_p, int16_t* counts, int counts_stride,
-                  const float* presence, const float* frequency, cudaStream_t s);
+struct SampleParams {
+  const float* logits;      // [B, ld]
+  uint32_t* seen;           // [rows, ceil(V/32)] bitmap of ids in the context, or null
+  int* out_tokens;          // [rows] local
+  int* peer_tokens;         // [rows] on piece 0 (may be == out_tokens / null)
+  int* history;             // [rows, hist_stride] token ring, or null
+  const int* hist_pos;      // [rows] write index into history
+  int* hist_pos_out;        // [rows] incremented copy
+  int hist_stride;
+  int vocab;
+  int ld;                   // row stride of logits (vocab padded to a GEMM tile)
+  float softcap;            // final-logit soft-capping (Gemma-2), 0 = off
+  const float* temperature; // [rows]
+  const float* top_p;       // [rows]
+  const int* top_k;         // [rows] (<= 0 or >= vocab = off), or null
+  const float* min_p;       // [rows] (<= 0 = off), or null
+  const float* rep_penalty; // [rows]
+  int16_t* counts;          // [rows, cstride] times each id was generated (saturates at 32767), or null
+  int cstride;              // row stride of counts in ids (a multiple of 8)
+  const float* presence;    // [rows] presence penalty p (0 = off), or null
+  const float* frequency;   // [rows] frequency penalty f (0 = off), or null
+  const uint32_t* seeds;    // [rows]
+  const uint32_t* step;     // device step counter (rng stream), may be null
+  uint32_t* signal_flag;    // peer flag (token handoff) or null
+  uint32_t* signal_epoch;   // local epoch for the flag
+  uint32_t* done_counter;   // local, self-resetting
+  const int* row_map;       // optional [batch]: per-sequence state of logits row b lives at row row_map[b]; < 0 = skip the row
+};
+// samples logits rows 0 .. batch-1; -7 = a count table with a bad stride or alignment, -6 = a vocabulary too large
+int launch_sample(const SampleParams& p, int batch, cudaStream_t s);
 // CTAs per sequence (1, 2, 4 or 8) that launch_sample runs a batch at on a device with `sms` SMs; 0 = the vocabulary
 // does not fit in shared memory at any cluster size
 int sample_cluster_size(int batch, int vocab, int sms);

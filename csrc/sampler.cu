@@ -48,35 +48,6 @@ __device__ __forceinline__ uint32_t hash_u32(uint32_t x) {
   return x;
 }
 
-struct SampleParams {
-  const float* logits;      // [B, ld]
-  uint32_t* seen;           // [rows, ceil(V/32)] bitmap of ids in the context, or null
-  int* out_tokens;          // [rows] local
-  int* peer_tokens;         // [rows] on piece 0 (may be == out_tokens / null)
-  int* history;             // [rows, hist_stride] token ring, or null
-  const int* hist_pos;      // [rows] write index into history
-  int* hist_pos_out;        // [rows] incremented copy
-  int hist_stride;
-  int vocab;
-  int ld;                   // row stride of logits (vocab padded to a GEMM tile)
-  float softcap;            // final-logit soft-capping (Gemma-2), 0 = off
-  const float* temperature; // [rows]
-  const float* top_p;       // [rows]
-  const int* top_k;         // [rows] (<= 0 or >= vocab = off), or null
-  const float* min_p;       // [rows] (<= 0 = off), or null
-  const float* rep_penalty; // [rows]
-  int16_t* counts;          // [rows, cstride] times each id was generated (saturates at 32767), or null
-  int cstride;              // row stride of counts in ids (a multiple of 8)
-  const float* presence;    // [rows] presence penalty p (0 = off), or null
-  const float* frequency;   // [rows] frequency penalty f (0 = off), or null
-  const uint32_t* seeds;    // [rows]
-  const uint32_t* step;     // device step counter (rng stream), may be null
-  uint32_t* signal_flag;    // peer flag (token handoff) or null
-  uint32_t* signal_epoch;   // local epoch for the flag
-  uint32_t* done_counter;   // local, self-resetting
-  const int* row_map;       // optional [batch]: per-sequence state of logits row b lives at row row_map[b]; < 0 = skip the row
-};
-
 // logit -> (soft-cap) -> repetition penalty -> temperature
 __device__ __forceinline__ float transform(float l, bool is_seen, float pen, float inv_temp, float cap) {
   if (cap > 0.f) l = cap * tanhf(l / cap);
@@ -577,22 +548,11 @@ int sample_cluster_size(int batch, int vocab, int sms) {
   return cs;
 }
 
-int launch_sample(const float* logits, uint32_t* seen, int* out_tokens, int* peer_tokens, int* history,
-                  const int* hist_pos, int* hist_pos_out, int hist_stride, int batch, int vocab, int ld, float softcap,
-                  const float* temperature, const float* top_p, const float* rep_penalty, const uint32_t* seeds,
-                  const uint32_t* step, uint32_t* signal_flag, uint32_t* signal_epoch, uint32_t* done_counter,
-                  const int* row_map, const int* top_k, const float* min_p, int16_t* counts, int counts_stride,
-                  const float* presence, const float* frequency, cudaStream_t s) {
-  if (counts != nullptr && (counts_stride < vocab || counts_stride % 8 != 0 ||
-                            (reinterpret_cast<uintptr_t>(counts) & 7) != 0))
+int launch_sample(const SampleParams& p, int batch, cudaStream_t s) {
+  const int vocab = p.vocab;
+  if (p.counts != nullptr && (p.cstride < vocab || p.cstride % 8 != 0 ||
+                              (reinterpret_cast<uintptr_t>(p.counts) & 7) != 0))
     return -7;
-  SampleParams p;
-  p.logits = logits; p.seen = seen; p.out_tokens = out_tokens; p.peer_tokens = peer_tokens; p.history = history;
-  p.hist_pos = hist_pos; p.hist_pos_out = hist_pos_out; p.hist_stride = hist_stride; p.vocab = vocab; p.ld = ld; p.softcap = softcap;
-  p.temperature = temperature; p.top_p = top_p; p.top_k = top_k; p.min_p = min_p; p.rep_penalty = rep_penalty;
-  p.counts = counts; p.cstride = counts_stride; p.presence = presence; p.frequency = frequency;
-  p.seeds = seeds; p.step = step;
-  p.signal_flag = signal_flag; p.signal_epoch = signal_epoch; p.done_counter = done_counter; p.row_map = row_map;
   if (sample_cluster_size(1, vocab, 0) == 0) return -6;
   static int sm_count[64] = {};
   int dev = 0;

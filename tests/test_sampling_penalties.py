@@ -100,9 +100,9 @@ def test_sample_reference_applies_penalties_after_repetition_penalty():
     assert torch.equal(a, b) and torch.equal(a, d)
 
 
-def test_cpu_engine_counts_generated_tokens_only():
-    """the CPU backend's per-sequence counts are the histogram of the generated tokens; prompt tokens are not counted,
-    so a penalty changes nothing for the first token"""
+def test_cpu_sequence_sampler_counts_generated_tokens_only():
+    """the CPU backend's per-sequence counts (held by each sequence's ``SequenceSampler``) are the histogram of the
+    generated tokens; prompt tokens are not counted, so a penalty changes nothing for the first token"""
     eng = Engine("tiny-llama", device="cpu", max_batch=2, max_seq_len=64)
     runner = eng.runner
     prompt = [7, 7, 7, 3, 3, 9]
@@ -113,7 +113,8 @@ def test_cpu_engine_counts_generated_tokens_only():
     hist = {}
     for t in pen:
         hist[t] = hist.get(t, 0) + 1
-    assert runner.state[0]["counts"] == hist
+    counts = runner.state[0]["sampler"].counts[0]
+    assert {int(t): int(counts[t]) for t in counts.nonzero()} == hist
     assert sum(hist.values()) == len(pen) == 10
     assert plain[0] == pen[0]                       # counts start empty: the prompt is not penalised
     assert plain != pen                             # and the penalties do act on generated tokens
