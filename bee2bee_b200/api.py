@@ -108,6 +108,7 @@ class ChatRequest(BaseModel):
     min_p: Optional[float] = None     # keep tokens with p >= min_p * p_max; absent = off
     presence_penalty: Optional[float] = None    # in [-2, 2], subtracted from every generated token; absent = off
     frequency_penalty: Optional[float] = None   # in [-2, 2], times each generated token's count; absent = off
+    logit_bias: Optional[Dict[str, float]] = None   # token id (decimal string) -> bias in [-100, 100]; absent = off
 
 
 @app.get("/")
@@ -210,10 +211,10 @@ async def chat(req: ChatRequest):
         return {"status": "error", "message": "node not started"}
     params = {"prompt": req.prompt, "max_new_tokens": req.max_new_tokens or 2048,
               "temperature": 0.7 if req.temperature is None else req.temperature}
-    filters = sampling_filters({"top_k": req.top_k, "min_p": req.min_p, "presence_penalty": req.presence_penalty,
-                                "frequency_penalty": req.frequency_penalty})
-    params.update(filters)
     try:
+        filters = sampling_filters({"top_k": req.top_k, "min_p": req.min_p, "presence_penalty": req.presence_penalty,
+                                    "frequency_penalty": req.frequency_penalty, "logit_bias": req.logit_bias})
+        params.update(filters)
         t0 = time.time()
         want_local = req.provider_id in (None, "local", node.peer_id)
         svc = None

@@ -16,11 +16,12 @@ import itertools
 import os
 import collections
 import queue
+import re
 import statistics
 import threading
 import time
 from dataclasses import dataclass, field, fields
-from typing import Callable, Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Mapping, Optional, Sequence
 
 import numpy as np
 import torch
@@ -29,6 +30,35 @@ from ..models.config import ModelConfig, resolve_config, split_layers
 from ..models.torch_ref import SequenceSampler, TorchPiece
 from ..models.weights import load_or_init
 from .kv import PAGE, PageAllocator
+
+
+LOGIT_BIAS_MAX = 1024       # entries one request's logit_bias may hold (the width of the sampler's bias tables)
+LOGIT_BIAS_LIMIT = 100.0    # |bias| bound, as in OpenAI's API
+
+
+def parse_logit_bias(obj: Optional[Mapping]) -> Dict[int, float]:
+    """A request's ``logit_bias`` as the engine takes it: int token id -> float bias.  On the wire it is a JSON object
+    whose keys are decimal strings (OpenAI's shape); int keys are taken as they are.  None or an empty map = off.
+    Raises ``ValueError`` for a key that is not a decimal integer, for two keys that name the same id ("5" and "05")
+    and for a value that is not a number; ranges are checked by ``SamplerControls.validate``."""
+    if obj is None:
+        return {}
+    if not isinstance(obj, Mapping):
+        raise ValueError(f"logit_bias must be a map of token id -> bias, got {type(obj).__name__}")
+    out: Dict[int, float] = {}
+    for k, v in obj.items():
+        if isinstance(k, str) and re.fullmatch(r"[+-]?[0-9]+", k):
+            tid = int(k)
+        elif isinstance(k, (int, np.integer)) and not isinstance(k, bool):
+            tid = int(k)
+        else:
+            raise ValueError(f"logit_bias keys must be integer token ids, got {k!r}")
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)):
+            raise ValueError(f"logit_bias[{k!r}] must be a number, got {v!r}")
+        if tid in out:
+            raise ValueError(f"logit_bias names token id {tid} twice")
+        out[tid] = float(v)
+    return out
 
 
 @dataclass(kw_only=True)
@@ -42,9 +72,13 @@ class SamplerControls:
     min_p: float = 0.0                 # after top-p keep tokens with p >= min_p * p_max; 0 = off
     presence_penalty: float = 0.0      # subtracted from every token generated so far (prompt excluded); 0 = off
     frequency_penalty: float = 0.0     # times the token's generated count, subtracted too; 0 = off
+    # token id -> bias added to its logit after soft-cap, before the penalties; empty = off.  -100 makes a token
+    # negligible, not impossible.
+    logit_bias: Mapping[int, float] = field(default_factory=dict)
 
-    def validate(self) -> None:
-        """Raise ``ValueError`` for a control outside the range the sampler defines."""
+    def validate(self, vocab_size: Optional[int] = None) -> None:
+        """Raise ``ValueError`` for a control outside the range the sampler defines; with ``vocab_size``, also for a
+        ``logit_bias`` id outside the vocabulary."""
         if not self.top_k >= 0:
             raise ValueError(f"top_k must be >= 0 (0 = off), got {self.top_k}")
         if not 0.0 <= self.min_p <= 1.0:
@@ -53,6 +87,17 @@ class SamplerControls:
             v = getattr(self, name)
             if not -2.0 <= v <= 2.0:          # also refuses NaN and +-inf
                 raise ValueError(f"{name} must be a finite value in [-2, 2] (0 = off), got {v}")
+        if len(self.logit_bias) > LOGIT_BIAS_MAX:
+            raise ValueError(f"logit_bias holds {len(self.logit_bias)} entries; at most {LOGIT_BIAS_MAX} are allowed")
+        for k, v in self.logit_bias.items():
+            if isinstance(k, bool) or not isinstance(k, (int, np.integer)):
+                raise ValueError(f"logit_bias keys must be integer token ids, got {k!r}")
+            if k < 0 or (vocab_size is not None and k >= vocab_size):
+                raise ValueError(f"logit_bias id {k} lies outside the vocabulary"
+                                 + (f" of {vocab_size} ids" if vocab_size is not None else ""))
+            if (isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating))
+                    or not -LOGIT_BIAS_LIMIT <= v <= LOGIT_BIAS_LIMIT):     # also refuses NaN and +-inf
+                raise ValueError(f"logit_bias[{k}] must be a finite value in [-100, 100], got {v}")
 
     def controls(self) -> Dict[str, object]:
         """The controls alone, as keyword arguments for another ``SamplerControls``."""
@@ -236,7 +281,7 @@ class Engine:
     def submit(self, prompt_ids: Sequence[int], params: Optional[SamplingParams] = None,
                on_token: Optional[Callable[[int], None]] = None) -> Request:
         params = params or SamplingParams()
-        params.validate()
+        params.validate(self.cfg.vocab_size)
         ids = list(prompt_ids)[-(self.max_seq_len - 1):] or [max(self.cfg.bos_token_id, 0)]
         budget = self.max_seq_len - len(ids)
         if params.max_new_tokens > budget:

@@ -31,7 +31,7 @@ from ..models.config import UNITS_PER_LAYER, ModelConfig, piece_units, unit_laye
 from ..models.native import BatchMeta, NativePiece
 from ..models.weights import load_or_init
 from ..parallel.mesh import F_TOK_DONE, MeshComm
-from .core import SamplerControls
+from .core import LOGIT_BIAS_MAX, SamplerControls
 from .kv import PAGE
 
 
@@ -46,10 +46,20 @@ class SeqInit(SamplerControls):
 
 
 # The sampler's per-slot rows on the device, as (SeqInit field, ``ops.sample`` keyword) in the row order of the fp32
-# block and of the int32 block.  Every field is a contiguous row, and so is any slot range of it.
+# block and of the int32 block.  Every field is a contiguous row, and so is any slot range of it.  The logit_bias row
+# holds the slot's number of bias entries: admission rewrites it, so a reused slot never keeps an earlier bias.
 SAMPLER_F32_ROWS = (("temperature", "temperature"), ("top_p", "top_p"), ("repetition_penalty", "rep_penalty"),
                     ("min_p", "min_p"), ("presence_penalty", "presence"), ("frequency_penalty", "frequency"))
-SAMPLER_I32_ROWS = (("seed", "seeds"), ("top_k", "top_k"))
+SAMPLER_I32_ROWS = (("seed", "seeds"), ("top_k", "top_k"), ("logit_bias", "bias_n"))
+
+
+def _i32_row_value(s: "SeqInit", field: str) -> int:
+    v = getattr(s, field)
+    if field == "seed":
+        return int(v) & 0x7FFFFFFF          # the seed keeps its low 31 bits
+    if field == "logit_bias":
+        return len(v)
+    return int(v)
 
 
 def _pow2_at_least(n: int, lo: int = 1) -> int:
@@ -146,12 +156,14 @@ class GpuRunner:
         idle = SamplerControls(temperature=0.0, top_p=1.0, repetition_penalty=1.0)
         self.sampler_f32 = torch.tensor([[getattr(idle, f)] * B for f, _ in SAMPLER_F32_ROWS], device=dev,
                                         dtype=torch.float32)
-        self.sampler_i32 = torch.zeros((len(SAMPLER_I32_ROWS), B), device=dev, dtype=i32)    # seed 0, top_k 0 = off
+        self.sampler_i32 = torch.zeros((len(SAMPLER_I32_ROWS), B), device=dev, dtype=i32)    # seed 0; top_k 0, no bias
         self.hist_pos = torch.zeros(B, device=dev, dtype=i32)
         self.step_ctr = torch.zeros(1, device=dev, dtype=i32)
         self.seen = torch.zeros((B, (cfg.vocab_size + 31) // 32), device=dev, dtype=i32)
         # times each id was generated per slot (presence / frequency penalties); read and written by the sampler only
         self.counts = ops.counts_table(B, cfg.vocab_size, dev) if self.last else None
+        # logit bias ids / values per slot; a slot reads the first ``bias_n`` entries of its row (last piece only)
+        self.bias_ids, self.bias_vals = (ops.logit_bias_table(B, LOGIT_BIAS_MAX, dev) if self.last else (None, None))
         self.tok_local = torch.zeros(B, device=dev, dtype=i32)     # last rank's own copy of sampled ids
         self.graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self._pf: Dict[tuple, dict] = {}           # prefill state (staging + graph) per bucket
@@ -195,7 +207,8 @@ class GpuRunner:
         """``ops.sample`` keyword arguments of the per-slot state of slots [lo, hi)."""
         kw = {k: self.sampler_f32[r, lo:hi] for r, (_, k) in enumerate(SAMPLER_F32_ROWS)}
         kw.update({k: self.sampler_i32[r, lo:hi] for r, (_, k) in enumerate(SAMPLER_I32_ROWS)})
-        return dict(kw, seen=self.seen[lo:hi], counts=self.counts[lo:hi], hist_pos=self.hist_pos[lo:hi])
+        return dict(kw, seen=self.seen[lo:hi], counts=self.counts[lo:hi], hist_pos=self.hist_pos[lo:hi],
+                    bias_ids=self.bias_ids[lo:hi], bias_vals=self.bias_vals[lo:hi])
 
     def _reset_sampler_state(self, rows: Optional[torch.Tensor] = None) -> None:
         """Clear what the sampler accumulates per slot (history write position, seen bitmap, generated-token counts)
@@ -268,15 +281,23 @@ class GpuRunner:
             bt_np[i, :len(s.pages)] = s.pages
         bt_host = torch.from_numpy(bt_np)
         fl_host = torch.tensor([[getattr(s, f) for s in seqs] for f, _ in SAMPLER_F32_ROWS], dtype=torch.float32)
-        # the seed keeps its low 31 bits
-        int_host = torch.tensor([[int(getattr(s, f)) & 0x7FFFFFFF if f == "seed" else int(getattr(s, f)) for s in seqs]
-                                 for f, _ in SAMPLER_I32_ROWS], dtype=i32)
+        int_host = torch.tensor([[_i32_row_value(s, f) for s in seqs] for f, _ in SAMPLER_I32_ROWS], dtype=i32)
         rows = torch.tensor([s.slot for s in seqs], dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
         self.block_table.index_copy_(0, rows, bt_host.pin_memory().to(dev, non_blocking=True))
         self.sampler_f32.index_copy_(1, rows, fl_host.pin_memory().to(dev, non_blocking=True))
         self.sampler_i32.index_copy_(1, rows, int_host.pin_memory().to(dev, non_blocking=True))
         self._reset_sampler_state(rows)
         self.h2d_bytes += bt_host.numel() * 4 + fl_host.numel() * 4 + int_host.numel() * 4 + S * 8
+        if self.last and any(s.logit_bias for s in seqs):
+            # only the entries of the biased sequences travel, scattered into their slots' rows in one copy per table
+            dst = np.concatenate([s.slot * LOGIT_BIAS_MAX + np.arange(len(s.logit_bias)) for s in seqs if s.logit_bias])
+            ids = np.concatenate([np.fromiter(s.logit_bias.keys(), np.int32) for s in seqs if s.logit_bias])
+            vals = np.concatenate([np.fromiter(s.logit_bias.values(), np.float32) for s in seqs if s.logit_bias])
+            dst_d = torch.from_numpy(dst).pin_memory().to(dev, non_blocking=True)
+            self.bias_ids.view(-1).index_copy_(0, dst_d, torch.from_numpy(ids).pin_memory().to(dev, non_blocking=True))
+            self.bias_vals.view(-1).index_copy_(0, dst_d,
+                                                torch.from_numpy(vals).pin_memory().to(dev, non_blocking=True))
+            self.h2d_bytes += dst.nbytes + ids.nbytes + vals.nbytes
         if self.last:
             flat = np.concatenate([np.asarray(s.prompt, dtype=np.int32) for s in seqs])
             owner = np.repeat(np.asarray([s.slot for s in seqs], dtype=np.int32), [len(s.prompt) for s in seqs])

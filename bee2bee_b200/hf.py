@@ -7,7 +7,7 @@
                                                greedy when temperature <= 0, stop-word cut;
                                                optional top_k / min_p, off by default: transformers'
                                                implicit top_k=50 is not applied; optional presence /
-                                               frequency penalties, off by default)
+                                               frequency penalties and logit_bias, off by default)
     export_torchscript / export_onnx          (over the plain-torch module of the model)
     load_dataset / preprocess_examples
     build_layer_partial (== build_distilbert_partial generalised to decoder LMs: only the
@@ -112,14 +112,15 @@ def unload_model(model_name: str) -> int:
 
 def generate_text(model: LoadedModel, tokenizer, device: str, prompt: str, max_new_tokens: int = 32,
                   temperature: float = 0.7, return_full_text: bool = True, return_ids: bool = False, top_k: int = 0,
-                  min_p: float = 0.0, presence_penalty: float = 0.0, frequency_penalty: float = 0.0):
+                  min_p: float = 0.0, presence_penalty: float = 0.0, frequency_penalty: float = 0.0,
+                  logit_bias: Optional[Dict[int, float]] = None):
     """Non-streaming path: temperature + do_sample only (no top-p / repetition penalty), returns
-    prompt + completion like the reference (hf.py:35-44).  ``top_k`` / ``min_p`` and the presence / frequency
-    penalties are off unless given."""
+    prompt + completion like the reference (hf.py:35-44).  ``top_k`` / ``min_p``, the presence / frequency
+    penalties and ``logit_bias`` (token id -> bias) are off unless given."""
     ids = tokenizer.encode(prompt)
     sp = SamplingParams(max_new_tokens=max_new_tokens, temperature=temperature, top_p=1.0, repetition_penalty=1.0,
                         top_k=top_k, min_p=min_p, presence_penalty=presence_penalty,
-                        frequency_penalty=frequency_penalty)
+                        frequency_penalty=frequency_penalty, logit_bias=dict(logit_bias or {}))
     req = model.engine.submit(ids, sp)
     try:
         req.wait(timeout=600)
@@ -133,10 +134,11 @@ def generate_text(model: LoadedModel, tokenizer, device: str, prompt: str, max_n
 
 def generate_text_stream(model: LoadedModel, tokenizer, device: str, prompt: str, max_new_tokens: int = 512,
                          temperature: float = 0.7, top_k: int = 0, min_p: float = 0.0, presence_penalty: float = 0.0,
-                         frequency_penalty: float = 0.0) -> Iterator[str]:
+                         frequency_penalty: float = 0.0,
+                         logit_bias: Optional[Dict[int, float]] = None) -> Iterator[str]:
     """Streaming path (hf.py:46-136): transcript -> chat template, rep. penalty 1.15, top_p 0.95
-    (greedy when temperature <= 0), yields text deltas, stops at the first stop word.  ``top_k`` / ``min_p`` and the
-    presence / frequency penalties are off unless given."""
+    (greedy when temperature <= 0), yields text deltas, stops at the first stop word.  ``top_k`` / ``min_p``, the
+    presence / frequency penalties and ``logit_bias`` are off unless given."""
     messages = parse_transcript(prompt)
     try:
         rendered = tokenizer.apply_chat_template(messages, add_generation_prompt=True)
@@ -146,7 +148,7 @@ def generate_text_stream(model: LoadedModel, tokenizer, device: str, prompt: str
     q: "queue.Queue[Optional[int]]" = queue.Queue()
     sp = SamplingParams(max_new_tokens=max_new_tokens, temperature=temperature, top_p=0.95, repetition_penalty=1.15,
                         top_k=top_k, min_p=min_p, presence_penalty=presence_penalty,
-                        frequency_penalty=frequency_penalty)
+                        frequency_penalty=frequency_penalty, logit_bias=dict(logit_bias or {}))
     req = model.engine.submit(ids, sp, on_token=q.put)
     emitted, toks = "", []
     try:

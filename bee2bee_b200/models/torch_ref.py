@@ -146,15 +146,21 @@ COUNT_MAX = 32767       # generated-token counts saturate here (the sampler's in
 def sample_reference(logits: torch.Tensor, seen: Optional[torch.Tensor], temperature: float, top_p: float,
                      rep_penalty: float, generator: Optional[torch.Generator] = None, top_k: int = 0,
                      min_p: float = 0.0, counts: Optional[torch.Tensor] = None, presence: float = 0.0,
-                     frequency: float = 0.0) -> torch.Tensor:
-    """HF-processor semantics (repetition penalty -> presence / frequency penalty -> temperature -> top-k -> top-p ->
-    min-p -> multinomial / greedy when temperature <= 0), cf. /root/reference/bee2bee/hf.py:91-105.
+                     frequency: float = 0.0, bias: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> torch.Tensor:
+    """HF-processor semantics (logit bias -> repetition penalty -> presence / frequency penalty -> temperature -> top-k
+    -> top-p -> min-p -> multinomial / greedy when temperature <= 0), cf. /root/reference/bee2bee/hf.py:91-105.
+    ``bias`` = (ids int64 [n], values fp32 [n]): every row's logit of ids[j] gains values[j] in fp32 (vLLM's and
+    OpenAI's ``logit_bias``; ids unique); the other ids are untouched.  The logits arrive soft-capped, so the bias
+    follows soft-cap and the repetition penalty sees the biased logit.
     logits [B, V] fp32; seen [B, V] bool of ids already in the context.  ``top_k`` keeps the tokens at least as likely
     as the k-th (ties kept; <= 0 or >= V = off); top-p then sees the top-k survivors renormalised; ``min_p`` keeps
     p >= min_p * p_max (<= 0 = off).  ``counts`` [B, V] holds how often each id was generated (prompt excluded); where
     it is positive, l = (l - frequency * c) - presence in fp32, as vLLM / OpenAI define the two penalties (0 = off);
     greedy rows are penalised too."""
     l = logits.float().clone()
+    if bias is not None and bias[0].numel() > 0:
+        ids, vals = bias
+        l[:, ids] = l[:, ids] + vals.to(torch.float32)
     if seen is not None and rep_penalty != 1.0:
         pen = torch.where(l > 0, l / rep_penalty, l * rep_penalty)
         l = torch.where(seen, pen, l)
@@ -182,13 +188,17 @@ def sample_reference(logits: torch.Tensor, seen: Optional[torch.Tensor], tempera
 
 class SequenceSampler:
     """One sequence's sampling on the CPU: its controls (any ``engine.core.SamplerControls``), its generator, the ids
-    in its context (repetition penalty) and how often each id was generated (presence / frequency penalties)."""
+    in its context (repetition penalty), how often each id was generated (presence / frequency penalties) and its
+    logit bias."""
 
     def __init__(self, controls, vocab: int, prompt: Iterable[int], generator: torch.Generator):
         self.controls, self.generator = controls, generator
         self.seen = torch.zeros(1, vocab, dtype=torch.bool)
         self.seen[0, torch.tensor(sorted({int(t) for t in prompt}), dtype=torch.long)] = True
         self.counts = torch.zeros(1, vocab, dtype=torch.int32)       # generated tokens only, saturating at COUNT_MAX
+        lb = controls.logit_bias
+        self.bias = ((torch.tensor([int(t) for t in lb], dtype=torch.long),
+                      torch.tensor([float(v) for v in lb.values()], dtype=torch.float32)) if lb else None)
 
     def draw(self, logits: torch.Tensor) -> int:
         """The next id from ``logits`` [>= vocab] of the sequence's last position; it is then seen and counted."""
@@ -197,7 +207,7 @@ class SequenceSampler:
         tok = int(sample_reference(logits[None, :self.seen.shape[1]].cpu(), self.seen, c.temperature, c.top_p,
                                    c.repetition_penalty, self.generator, top_k=c.top_k, min_p=c.min_p,
                                    counts=self.counts if penalised else None, presence=c.presence_penalty,
-                                   frequency=c.frequency_penalty))
+                                   frequency=c.frequency_penalty, bias=self.bias))
         self.seen[0, tok] = True
         self.counts[0, tok] = min(int(self.counts[0, tok]) + 1, COUNT_MAX)
         return tok

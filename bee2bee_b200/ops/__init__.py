@@ -399,24 +399,35 @@ def get_attn_tc_min_q() -> int:
 # ---------------------------------------------------------------------- sampler
 def sample(logits, out_tokens, *, seen=None, temperature=None, top_p=None, rep_penalty=None, seeds=None, step=None,
            peer_tokens=0, history=0, hist_pos=None, hist_stride=0, signal_flag=0, signal_epoch=0, done_counter=0,
-           vocab=0, softcap=0.0, row_map=0, top_k=None, min_p=None, counts=None, presence=None, frequency=None):
+           vocab=0, softcap=0.0, row_map=0, top_k=None, min_p=None, counts=None, presence=None, frequency=None,
+           bias_ids=None, bias_vals=None, bias_n=None):
     """``row_map``: device address of int32 [rows of logits] mapping each logits row to its batch row (< 0 = skip).
     ``top_k`` (int32, <= 0 or >= vocab = off) and ``min_p`` (fp32, <= 0 = off) hold one entry per batch row, like
     ``temperature``; None turns the filter off for every row.
     ``counts`` (int16 [batch rows, cstride], see ``counts_table``) holds how often each id was generated per row; the
     sampler adds one to the drawn id's count (saturating at 32767).  ``presence`` / ``frequency`` (fp32, one entry per
     batch row, 0 = off) subtract ``frequency * c + presence`` from every logit whose count c is positive; they need
-    ``counts``."""
+    ``counts``.
+    ``bias_ids`` (int32) / ``bias_vals`` (fp32) [batch rows, width] (see ``logit_bias_table``) and ``bias_n`` (int32,
+    one entry per batch row, 0 = off) give each row a logit bias: ``bias_vals[r, j]`` is added to the logit of id
+    ``bias_ids[r, j]`` for j < min(bias_n[r], width), after soft-cap and before the penalties.  The ids of a row must
+    be unique; ids outside [0, vocab) are ignored.  The three go together."""
     native().sample(logits, seen, out_tokens, peer_tokens, history, hist_pos, hist_stride, vocab, softcap,
                     temperature, top_p,
                     rep_penalty, seeds, step, signal_flag, signal_epoch, done_counter, row_map, top_k, min_p,
-                    counts, presence, frequency)
+                    counts, presence, frequency, bias_ids, bias_vals, bias_n)
     return out_tokens
 
 
 def counts_table(rows, vocab, device):
     """Zeroed int16 [rows, vocab rounded up to 8] table of generated-token counts for ``sample(counts=...)``."""
     return torch.zeros((rows, (vocab + 7) // 8 * 8), dtype=torch.int16, device=device)
+
+
+def logit_bias_table(rows, width, device):
+    """Zeroed int32 ids and fp32 values, each [rows, width], for ``sample(bias_ids=..., bias_vals=...)``."""
+    return (torch.zeros((rows, width), dtype=torch.int32, device=device),
+            torch.zeros((rows, width), dtype=torch.float32, device=device))
 
 
 def mark_seen(ids, seq_of, seen, vocab):

@@ -467,9 +467,14 @@ class P2PNode:
     async def _handle_gen_request(self, conn: Connection, data: Dict[str, Any]) -> None:
         rid = P.request_id_of(data) or new_id("req")
         model = data.get("model")
+        try:
+            filters = sampling_filters(data)
+        except ValueError as exc:             # a malformed logit_bias: refused before it reaches a service
+            await self._send(conn, P.msg(P.GEN_RESULT, rid=rid, error=f"bad_request: {exc}"))
+            return
         params = {"prompt": data.get("prompt"),
                   "max_new_tokens": int(data.get("max_new_tokens") or data.get("max_tokens") or 2048),
-                  "temperature": data.get("temperature", 0.7), **sampling_filters(data)}
+                  "temperature": data.get("temperature", 0.7), **filters}
         svc = self._find_local_service(data.get("svc", "hf"), model)
         if svc is not None:
             # run as a task so this peer's reader keeps draining pings / other requests
@@ -676,11 +681,12 @@ class P2PNode:
                                  on_chunk: Optional[Callable[[str], None]] = None,
                                  timeout: float = DEFAULT_GEN_TIMEOUT, top_k: Optional[int] = None,
                                  min_p: Optional[float] = None, presence_penalty: Optional[float] = None,
-                                 frequency_penalty: Optional[float] = None) -> Dict[str, Any]:
-        """``top_k`` / ``min_p`` / ``presence_penalty`` / ``frequency_penalty``: optional sampling controls (None =
-        off), passed on only when set."""
+                                 frequency_penalty: Optional[float] = None,
+                                 logit_bias: Optional[Dict[int, float]] = None) -> Dict[str, Any]:
+        """``top_k`` / ``min_p`` / ``presence_penalty`` / ``frequency_penalty`` / ``logit_bias``: optional sampling
+        controls (None = off; an empty ``logit_bias`` too), passed on only when set."""
         filters = sampling_filters({"top_k": top_k, "min_p": min_p, "presence_penalty": presence_penalty,
-                                    "frequency_penalty": frequency_penalty})
+                                    "frequency_penalty": frequency_penalty, "logit_bias": logit_bias})
         params = {"prompt": prompt, "max_new_tokens": max_new_tokens, "temperature": temperature, **filters}
         if provider_id == self.peer_id:
             svc = self._find_local_service(None, model_name)

@@ -19,7 +19,7 @@ import base64
 import json
 import threading
 import time
-from typing import Any, Dict, Iterator, List, Optional
+from typing import Any, Dict, Iterator, List, Mapping, Optional
 
 import torch
 
@@ -132,10 +132,13 @@ class MeshPipelineService(BaseService):
     async def agenerate(self, prompt_ids: List[int], max_new: int, temperature: float, top_p: float = 1.0,
                         rep: float = 1.0, on_token=None, seed: int = 0, top_k: int = 0,
                         min_p: float = 0.0, presence_penalty: float = 0.0,
-                        frequency_penalty: float = 0.0) -> List[int]:
+                        frequency_penalty: float = 0.0, logit_bias: Optional[Mapping[int, float]] = None) -> List[int]:
         session = new_id("sess")
         controls = SamplerControls(temperature=temperature, top_p=top_p, repetition_penalty=rep, top_k=top_k,
-                                   min_p=min_p, presence_penalty=presence_penalty, frequency_penalty=frequency_penalty)
+                                   min_p=min_p, presence_penalty=presence_penalty, frequency_penalty=frequency_penalty,
+                                   logit_bias=dict(logit_bias or {}))
+        if controls.logit_bias:      # the ids must lie in the vocabulary (the other controls are taken as given)
+            SamplerControls(logit_bias=controls.logit_bias).validate(self.cfg.vocab_size)
         sampler = SequenceSampler(controls, self.cfg.vocab_size, prompt_ids, torch.Generator().manual_seed(seed))
         out: List[int] = []
         try:

@@ -311,6 +311,7 @@ class SupervisedEngine:
         from ..engine.core import Request, SamplingParams
 
         params = params or SamplingParams()
+        params.validate(self.cfg.vocab_size)      # refused here, as by Engine.submit, rather than inside the worker
         r = Request(next(self._ids), list(prompt_ids), params, on_token, t_submit=time.time())
         if self.broken:
             r.error, r.finish_reason, r.t_done = self.broken, "error", time.time()
@@ -321,6 +322,7 @@ class SupervisedEngine:
         try:
             p = dict(params.__dict__)
             p["stop_token_ids"] = list(p.get("stop_token_ids") or ())
+            p["logit_bias"] = dict(p.get("logit_bias") or {})          # JSON turns its int keys into strings
             self._send({"op": "submit", "id": r.rid, "prompt_ids": r.prompt_ids, "params": p,
                         "stream": on_token is not None})
         except Exception as exc:
@@ -430,6 +432,7 @@ def _worker(a: argparse.Namespace) -> int:
                 if op == "submit":
                     p = dict(msg["params"])
                     p["stop_token_ids"] = tuple(p.get("stop_token_ids") or ())
+                    p["logit_bias"] = {int(k): v for k, v in (p.get("logit_bias") or {}).items()}
                     rid = msg["id"]
                     cb = (lambda t, i=rid: toks.put((i, int(t)))) if msg.get("stream") else None
                     live[rid] = eng.submit(msg["prompt_ids"], SamplingParams(**p), on_token=cb)

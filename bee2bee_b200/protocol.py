@@ -78,7 +78,8 @@ def service_announce(service: str, meta: Dict[str, Any]) -> Dict[str, Any]:
 def gen_request(rid: str, prompt: str, model: Optional[str] = None, svc: str = "hf", max_new_tokens: int = 2048,
                 temperature: float = 0.7, stream: bool = False, top_k: Optional[int] = None,
                 min_p: Optional[float] = None, presence_penalty: Optional[float] = None,
-                frequency_penalty: Optional[float] = None) -> Dict[str, Any]:
+                frequency_penalty: Optional[float] = None,
+                logit_bias: Optional[Dict[int, float]] = None) -> Dict[str, Any]:
     # both spellings are sent: the reference reads ``max_tokens`` but its requester writes
     # ``max_new_tokens`` (p2p_runtime.py:577 vs 822)
     m = msg(GEN_REQUEST, rid=rid, prompt=prompt, model=model, svc=svc, max_new_tokens=max_new_tokens,
@@ -92,6 +93,8 @@ def gen_request(rid: str, prompt: str, model: Optional[str] = None, svc: str = "
         m["presence_penalty"] = float(presence_penalty)
     if frequency_penalty is not None:
         m["frequency_penalty"] = float(frequency_penalty)
+    if logit_bias:
+        m["logit_bias"] = {str(int(k)): float(v) for k, v in logit_bias.items()}     # JSON keys: decimal strings
     return m
 
 

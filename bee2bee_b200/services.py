@@ -34,14 +34,20 @@ class ServiceError(Exception):
 
 
 def sampling_filters(params: Dict[str, Any]) -> Dict[str, Any]:
-    """The ``top_k`` / ``min_p`` / ``presence_penalty`` / ``frequency_penalty`` a request sets (absent or null = off),
-    as keyword arguments."""
+    """The ``top_k`` / ``min_p`` / ``presence_penalty`` / ``frequency_penalty`` / ``logit_bias`` a request sets (absent
+    or null = off; an empty ``logit_bias`` too), as keyword arguments.  ``logit_bias`` comes out with int keys;
+    ``ValueError`` for a malformed one (see ``engine.core.parse_logit_bias``)."""
+    from .engine.core import parse_logit_bias
+
     out: Dict[str, Any] = {}
     if params.get("top_k") is not None:
         out["top_k"] = int(params["top_k"])
     for name in ("min_p", "presence_penalty", "frequency_penalty"):
         if params.get(name) is not None:
             out[name] = float(params[name])
+    bias = parse_logit_bias(params.get("logit_bias"))
+    if bias:
+        out["logit_bias"] = bias
     return out
 
 
@@ -205,9 +211,10 @@ class EmbeddedOllama:
         opts = payload.get("options") or {}
         # top_k / min_p only when the request sets them: Ollama's own top_k default (40) is not applied.  Ollama (like
         # llama.cpp) treats top_k <= 0 and min_p <= 0 as off, so negative values mean off here too.  presence_penalty /
-        # frequency_penalty likewise only when present; negative values favour repetition, as in Ollama.
+        # frequency_penalty likewise only when present; negative values favour repetition, as in Ollama.  Ollama has no
+        # logit_bias option, so none is read from the options.
         filters = {k: (v if v > 0 else type(v)(0)) if k in ("top_k", "min_p") else v
-                   for k, v in sampling_filters(opts).items()}
+                   for k, v in sampling_filters({k: v for k, v in opts.items() if k != "logit_bias"}).items()}
         sp = SamplingParams(max_new_tokens=int(opts.get("num_predict", 128)),
                             temperature=float(opts.get("temperature", 0.8)), top_p=float(opts.get("top_p", 0.9)),
                             repetition_penalty=float(opts.get("repeat_penalty", 1.1)), **filters)
@@ -294,9 +301,11 @@ class OllamaService(BaseService):
         prompt = params.get("prompt")
         if not prompt:
             raise ServiceError("Missing prompt")
+        # the Ollama API has no logit_bias option: it is not sent
+        filters = sampling_filters({k: v for k, v in params.items() if k != "logit_bias"})
         return {"model": self.actual_model, "prompt": prompt, "stream": stream,
                 "options": {"num_predict": int(params.get("max_new_tokens") or params.get("max_tokens") or 2048),
-                            "temperature": float(params.get("temperature", 0.7) or 0.7), **sampling_filters(params)}}
+                            "temperature": float(params.get("temperature", 0.7) or 0.7), **filters}}
 
     def execute(self, params: Dict[str, Any]) -> Dict[str, Any]:
         payload = self._payload(params, stream=False)

@@ -388,7 +388,8 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
             const OptT& temperature, const OptT& top_p,
             const OptT& rep_penalty, const OptT& seeds, const OptT& step, int64_t signal_flag, int64_t signal_epoch,
             int64_t done_counter, int64_t row_map, const OptT& top_k, const OptT& min_p, const OptT& counts,
-            const OptT& presence, const OptT& frequency) {
+            const OptT& presence, const OptT& frequency, const OptT& bias_ids, const OptT& bias_vals,
+            const OptT& bias_n) {
   TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.stride(1) == 1, "logits: fp32");
   // top_k / min_p are per-sequence state like temperature: one entry per state row (logits row b reads row
   // row_map[b], or b without a row_map)
@@ -420,6 +421,25 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
                 "counts rows must hold the vocabulary (", V, " ids) at a row stride that is a multiple of 8 ids, "
                 "from an 8-byte aligned address; got ", c.size(1), " ids at stride ", c.stride(0));
   }
+  // logit bias: [state rows, width] int32 ids and fp32 values, and the entries in use per row (bias_n, like top_k)
+  const bool has_ids = bias_ids.has_value() && bias_ids->defined();
+  const bool has_vals = bias_vals.has_value() && bias_vals->defined();
+  const bool has_bias = bias_n.has_value() && bias_n->defined();
+  TORCH_CHECK(has_ids == has_bias && has_vals == has_bias, "bias_ids, bias_vals and bias_n go together");
+  if (has_bias) {
+    check_row_param(bias_n, at::kInt, "bias_n");
+    auto check_table = [&](const Tensor& t, at::ScalarType dtype, const char* name) {
+      TORCH_CHECK(t.scalar_type() == dtype && t.device() == logits.device() && t.dim() == 2 && t.is_contiguous(),
+                  name, " must be a contiguous 2-D ", dtype == at::kInt ? "int32" : "float32",
+                  " tensor on the logits' device");
+      TORCH_CHECK(t.size(0) == state_rows, name, " has ", t.size(0), " rows; expected one per state row (",
+                  state_rows, ")");
+    };
+    check_table(*bias_ids, at::kInt, "bias_ids");
+    check_table(*bias_vals, at::kFloat, "bias_vals");
+    TORCH_CHECK(bias_ids->size(1) == bias_vals->size(1), "bias_ids and bias_vals must have the same width; got ",
+                bias_ids->size(1), " and ", bias_vals->size(1));
+  }
   c10::cuda::CUDAGuard guard(logits.device());
   b2b::SampleParams p{};
   p.logits = reinterpret_cast<const float*>(logits.data_ptr());
@@ -441,6 +461,10 @@ void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, in
   p.cstride = has_counts ? static_cast<int>(counts->stride(0)) : 0;
   p.presence = ptr_or_null<const float>(presence);
   p.frequency = ptr_or_null<const float>(frequency);
+  p.bias_ids = ptr_or_null<const int>(bias_ids);
+  p.bias_vals = ptr_or_null<const float>(bias_vals);
+  p.bias_n = ptr_or_null<const int>(bias_n);
+  p.bias_stride = has_bias ? static_cast<int>(bias_ids->size(1)) : 0;
   p.seeds = ptr_or_null<const uint32_t>(seeds);
   p.step = ptr_or_null<const uint32_t>(step);
   p.signal_flag = as_ptr<uint32_t>(signal_flag);

@@ -66,6 +66,10 @@ struct SampleParams {
   int cstride;              // row stride of counts in ids (a multiple of 8)
   const float* presence;    // [rows] presence penalty p (0 = off), or null
   const float* frequency;   // [rows] frequency penalty f (0 = off), or null
+  const int* bias_ids;      // [rows, bias_stride] ids of the row's logit bias (unique within a row), or null
+  const float* bias_vals;   // [rows, bias_stride] bias added to the logit of bias_ids[row, j]
+  const int* bias_n;        // [rows] bias entries in use (0 = off; clamped to bias_stride), or null = off everywhere
+  int bias_stride;          // row stride of bias_ids / bias_vals in entries
   const uint32_t* seeds;    // [rows]
   const uint32_t* step;     // device step counter (rng stream), may be null
   uint32_t* signal_flag;    // peer flag (token handoff) or null

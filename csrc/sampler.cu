@@ -1,5 +1,6 @@
-// Fused sampler for sm_90a: repetition penalty (seen-token bitmap) -> presence / frequency
-// penalty (per-row counts of generated tokens) -> temperature -> top-k -> top-p -> min-p, each decided on a two-level radix histogram of the probability bits ->
+// Fused sampler for sm_90a: soft-cap -> logit bias (per-row id / value table) -> repetition penalty (seen-token
+// bitmap) -> presence / frequency penalty (per-row counts of generated tokens) -> temperature -> top-k -> top-p ->
+// min-p, each decided on a two-level radix histogram of the probability bits ->
 // multinomial draw (or argmax when temperature <= 0).  One cluster per sequence, logits are
 // fp32 [B, ld] as written by the lm_head GEMM.  The sampled id is stored locally (token ring,
 // history bitmap) and, on the last piece of a pipeline, straight into piece 0's token buffer on
@@ -14,6 +15,14 @@
 // when p or f is non-zero (row-uniform branch; a row with both off runs the unchanged phase-1 loop),
 // greedy rows included.  When a count table is given, the publishing thread increments the drawn
 // id's count (saturating); every CTA of the cluster has read its counts before the draw.
+// Logit bias (OpenAI / vLLM `logit_bias`; per row, bias_n = 0 = off) runs right after soft-cap, so the repetition
+// penalty's sign test sees the biased logit: l = l + b in round-to-nearest (__fadd_rn) for each of the row's first
+// min(bias_n, bias_stride) entries; other ids are untouched.  The ids of a row must be unique (the host guarantees
+// it); an id outside [0, V) lies in no CTA's slice and is ignored.  A biased row (row-uniform branch) stages its
+// bias in the CTA's shared-memory slice before phase 1 -- zero-filled, then each entry whose id the CTA owns is
+// scattered to its slot -- and phase 1 reads the slot before overwriting it with the transformed logit, so the
+// single max / argmax pass and every later phase are unchanged.  A row with bias_n = 0 runs the unchanged phase-1
+// loops.  Greedy rows are biased too.
 // After temperature the filters run in transformers' processor order, with e = exp(l - max):
 //   * top-k (k per row; k <= 0 or k >= V = off): K = the tokens whose e is at least the k-th
 //     largest e, ties at the k-th value kept.  K is decided on the same 22-bit key (top 22 bits
@@ -59,6 +68,16 @@ __device__ __forceinline__ float transform(float l, bool is_seen, float pen, flo
 __device__ __forceinline__ float transform_pf(float l, bool is_seen, int c, float pen, float pres, float freq,
                                              float inv_temp, float cap) {
   if (cap > 0.f) l = cap * tanhf(l / cap);
+  if (is_seen) l = l > 0.f ? l / pen : l * pen;
+  if (c > 0) l = __fsub_rn(__fsub_rn(l, __fmul_rn(freq, static_cast<float>(c))), pres);
+  return l * inv_temp;
+}
+
+// transform_pf() with the logit bias b added right after soft-cap (b = 0 for an unlisted id)
+__device__ __forceinline__ float transform_bias(float l, float b, bool is_seen, int c, float pen, float pres,
+                                                float freq, float inv_temp, float cap) {
+  if (cap > 0.f) l = cap * tanhf(l / cap);
+  l = __fadd_rn(l, b);
   if (is_seen) l = l > 0.f ? l / pen : l * pen;
   if (c > 0) l = __fsub_rn(__fsub_rn(l, __fmul_rn(freq, static_cast<float>(c))), pres);
   return l * inv_temp;
@@ -183,9 +202,49 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
     arrive();
   };
 
-  // ---- phase 1: L2 -> (soft-cap, penalty, temperature) -> shared memory; running max / argmax
+  const int nbias = p.bias_n ? min(p.bias_n[bb], p.bias_stride) : 0;
+
+  // ---- phase 1: L2 -> (soft-cap, bias, penalties, temperature) -> shared memory; running max / argmax
   float mx = -INFINITY; int amx = 0;
-  if (cnt != nullptr) {
+  if (nbias > 0) {
+    // biased row: stage the bias of the ids this CTA owns in its slice (0 for the others)
+    for (int j = tid; j < n; j += SAMP_THREADS) ebuf[j] = 0.f;
+    __syncthreads();
+    const int* bid = p.bias_ids + static_cast<size_t>(bb) * p.bias_stride;
+    const float* bval = p.bias_vals + static_cast<size_t>(bb) * p.bias_stride;
+    for (int j = tid; j < nbias; j += SAMP_THREADS) {
+      const int id = bid[j];
+      if (id >= lo && id < hi) ebuf[id - lo] = bval[j];
+    }
+    __syncthreads();
+    // 4 ids per iteration: their staged biases in one 16-byte shared load, their counts (penalised rows) in one
+    // aligned 8-byte load
+    auto take = [&](int i, float raw, float bias, uint32_t sw, int c) {
+      const float l = transform_bias(raw, bias, (sw >> (i & 31)) & 1u, c, pen, pres, freq, inv_temp, cap);
+      ebuf[i - lo] = l;
+      if (l > mx) { mx = l; amx = i; }
+    };
+    for (int q = tid; q < n4; q += SAMP_THREADS) {
+      const int i0 = lo + 4 * q;
+      float a[4];
+      if (vec_ok) {
+        const float4 va = *reinterpret_cast<const float4*>(logits + i0);
+        a[0] = va.x; a[1] = va.y; a[2] = va.z; a[3] = va.w;
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) a[k] = logits[i0 + k];
+      }
+      const float4 bv = reinterpret_cast<const float4*>(ebuf)[q];
+      const uint2 cw = cnt ? *reinterpret_cast<const uint2*>(cnt + i0) : make_uint2(0u, 0u);
+      const uint32_t sa = seen_r ? seen_r[i0 >> 5] : 0u;
+      take(i0, a[0], bv.x, sa, static_cast<int16_t>(cw.x & 0xFFFFu));
+      take(i0 + 1, a[1], bv.y, sa, static_cast<int16_t>(cw.x >> 16));
+      take(i0 + 2, a[2], bv.z, sa, static_cast<int16_t>(cw.y & 0xFFFFu));
+      take(i0 + 3, a[3], bv.w, sa, static_cast<int16_t>(cw.y >> 16));
+    }
+    for (int i = lo + 4 * n4 + tid; i < hi; i += SAMP_THREADS)
+      take(i, logits[i], ebuf[i - lo], seen_r ? seen_r[i >> 5] : 0u, cnt ? cnt[i] : 0);
+  } else if (cnt != nullptr) {
     // penalised row: 4 ids per iteration, their counts in one aligned 8-byte load
     auto take = [&](int i, float raw, uint32_t sw, int c) {
       const float l = transform_pf(raw, (sw >> (i & 31)) & 1u, c, pen, pres, freq, inv_temp, cap);

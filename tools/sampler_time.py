@@ -1,7 +1,9 @@
 """Time ``sample`` at B=32, V=128256 (Llama-3 vocabulary), T=0.7, repetition penalty 1.15, for these settings:
 off (top_p 0.95), top_k=50, top_k=50 with top_p=0.95, min_p=0.05; off with a count table (what the engine runs when a
 request sets no penalty: the table is only written); presence and frequency penalties 0.5 over a count table with a
-few hundred distinct ids per row, alone and with top_k=50.  The settings run in one process and alternate round by
+few hundred distinct ids per row, alone and with top_k=50; off with the logit-bias tables (every row's entry count 0:
+what the engine runs for a request without logit_bias); a 1024-entry logit bias per row (distinct random ids, biases
+in [-2, 2]).  The settings run in one process and alternate round by
 round, so clock and neighbour load drift hit all of them alike.  Prints the card and its power limit."""
 import os
 import subprocess
@@ -36,6 +38,10 @@ gen = torch.Generator(device="cpu").manual_seed(1)
 for b in range(B):
     ids = torch.randperm(V, generator=gen)[:400]
     counts[b, ids.to(dev)] = torch.randint(1, 13, (400,), generator=gen, dtype=torch.int16).to(dev)
+bias_ids, bias_vals = ops.logit_bias_table(B, 1024, dev)
+for b in range(B):
+    bias_ids[b] = torch.randperm(V, generator=gen)[:1024].to(dev, torch.int32)
+    bias_vals[b] = (torch.rand(1024, generator=gen) * 4.0 - 2.0).to(dev)
 
 
 def full(v, dtype=torch.float32):
@@ -51,6 +57,8 @@ rows = {
     "p=0.5 f=0.5": dict(top_p=full(0.95), counts=counts, presence=full(0.5), frequency=full(0.5)),
     "p=0.5 f=0.5 top_k=50": dict(top_p=full(0.95), top_k=full(50, torch.int32), min_p=full(0.0), counts=counts,
                                  presence=full(0.5), frequency=full(0.5)),
+    "off + bias tables": dict(top_p=full(0.95), bias_ids=bias_ids, bias_vals=bias_vals, bias_n=full(0, torch.int32)),
+    "logit_bias 1024": dict(top_p=full(0.95), bias_ids=bias_ids, bias_vals=bias_vals, bias_n=full(1024, torch.int32)),
 }
 
 
