@@ -412,10 +412,12 @@ def sample(logits, out_tokens, *, seen=None, temperature=None, top_p=None, rep_p
     one entry per batch row, 0 = off) give each row a logit bias: ``bias_vals[r, j]`` is added to the logit of id
     ``bias_ids[r, j]`` for j < min(bias_n[r], width), after soft-cap and before the penalties.  The ids of a row must
     be unique; ids outside [0, vocab) are ignored.  The three go together."""
-    native().sample(logits, seen, out_tokens, peer_tokens, history, hist_pos, hist_stride, vocab, softcap,
-                    temperature, top_p,
-                    rep_penalty, seeds, step, signal_flag, signal_epoch, done_counter, row_map, top_k, min_p,
-                    counts, presence, frequency, bias_ids, bias_vals, bias_n)
+    native().sample(logits=logits, out_tokens=out_tokens, seen=seen, temperature=temperature, top_p=top_p,
+                    rep_penalty=rep_penalty, seeds=seeds, step=step, peer_tokens=peer_tokens, history=history,
+                    hist_pos=hist_pos, hist_stride=hist_stride, signal_flag=signal_flag, signal_epoch=signal_epoch,
+                    done_counter=done_counter, vocab=vocab, softcap=softcap, row_map=row_map, top_k=top_k,
+                    min_p=min_p, counts=counts, presence=presence, frequency=frequency, bias_ids=bias_ids,
+                    bias_vals=bias_vals, bias_n=bias_n)
     return out_tokens
 
 

@@ -383,13 +383,14 @@ void attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, co
 }
 
 // ---------------------------------------------------------------------- sampler
-void sample(const Tensor& logits, const OptT& seen, const Tensor& out_tokens, int64_t peer_tokens,
-            int64_t history, const OptT& hist_pos, int64_t hist_stride, int64_t vocab, double softcap,
-            const OptT& temperature, const OptT& top_p,
-            const OptT& rep_penalty, const OptT& seeds, const OptT& step, int64_t signal_flag, int64_t signal_epoch,
-            int64_t done_counter, int64_t row_map, const OptT& top_k, const OptT& min_p, const OptT& counts,
-            const OptT& presence, const OptT& frequency, const OptT& bias_ids, const OptT& bias_vals,
-            const OptT& bias_n) {
+// bound keyword-only, with ops.sample's parameter names and no defaults: the optional per-row tensors share one type,
+// so a positional slip would still pass every check and sample with the wrong control
+void sample(const Tensor& logits, const Tensor& out_tokens, const OptT& seen, const OptT& temperature,
+            const OptT& top_p, const OptT& rep_penalty, const OptT& seeds, const OptT& step, int64_t peer_tokens,
+            int64_t history, const OptT& hist_pos, int64_t hist_stride, int64_t signal_flag, int64_t signal_epoch,
+            int64_t done_counter, int64_t vocab, double softcap, int64_t row_map, const OptT& top_k,
+            const OptT& min_p, const OptT& counts, const OptT& presence, const OptT& frequency,
+            const OptT& bias_ids, const OptT& bias_vals, const OptT& bias_n) {
   TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.stride(1) == 1, "logits: fp32");
   // top_k / min_p are per-sequence state like temperature: one entry per state row (logits row b reads row
   // row_map[b], or b without a row_map)
@@ -582,7 +583,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("use_tc") = -1);
   m.def("set_attn_tc_min_q", &set_attn_tc_min_q);
   m.def("get_attn_tc_min_q", &get_attn_tc_min_q);
-  m.def("sample", &sample);
+  m.def("sample", &sample, py::kw_only(), py::arg("logits"), py::arg("out_tokens"), py::arg("seen"),
+        py::arg("temperature"), py::arg("top_p"), py::arg("rep_penalty"), py::arg("seeds"), py::arg("step"),
+        py::arg("peer_tokens"), py::arg("history"), py::arg("hist_pos"), py::arg("hist_stride"),
+        py::arg("signal_flag"), py::arg("signal_epoch"), py::arg("done_counter"), py::arg("vocab"), py::arg("softcap"),
+        py::arg("row_map"), py::arg("top_k"), py::arg("min_p"), py::arg("counts"), py::arg("presence"),
+        py::arg("frequency"), py::arg("bias_ids"), py::arg("bias_vals"), py::arg("bias_n"));
   m.def("sample_cluster_size", &sample_cluster_size, py::arg("batch"), py::arg("vocab"));
   m.def("mark_seen", &mark_seen);
   m.def("set_decode_state", &set_decode_state);

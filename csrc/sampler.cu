@@ -8,21 +8,15 @@
 //
 // Semantics follow the reference's generation defaults (bee2bee/hf.py:91-105):
 // repetition_penalty 1.15, top_p 0.95, do_sample iff temperature > 0, greedy otherwise.
-// Presence / frequency penalties (vLLM / OpenAI; per row, 0 = off) run after the repetition penalty:
-// with c the number of times the id has been generated for the row (prompt excluded; an int16
-// table that saturates at 32767), l = (l - f c) - p when c > 0, in explicit round-to-nearest steps
-// (no FMA contraction, so an fp32 reference reproduces it bit for bit).  A row reads its counts only
-// when p or f is non-zero (row-uniform branch; a row with both off runs the unchanged phase-1 loop),
-// greedy rows included.  When a count table is given, the publishing thread increments the drawn
-// id's count (saturating); every CTA of the cluster has read its counts before the draw.
 // Logit bias (OpenAI / vLLM `logit_bias`; per row, bias_n = 0 = off) runs right after soft-cap, so the repetition
-// penalty's sign test sees the biased logit: l = l + b in round-to-nearest (__fadd_rn) for each of the row's first
-// min(bias_n, bias_stride) entries; other ids are untouched.  The ids of a row must be unique (the host guarantees
-// it); an id outside [0, V) lies in no CTA's slice and is ignored.  A biased row (row-uniform branch) stages its
-// bias in the CTA's shared-memory slice before phase 1 -- zero-filled, then each entry whose id the CTA owns is
-// scattered to its slot -- and phase 1 reads the slot before overwriting it with the transformed logit, so the
-// single max / argmax pass and every later phase are unchanged.  A row with bias_n = 0 runs the unchanged phase-1
-// loops.  Greedy rows are biased too.
+// penalty's sign test sees the biased logit: l = l + b for each of the row's first min(bias_n, bias_stride) entries;
+// other ids are untouched.  The ids of a row must be unique (the host guarantees it); an id outside [0, V) lies in no
+// CTA's slice and is ignored.
+// Presence / frequency penalties (vLLM / OpenAI; per row, 0 = off) run after the repetition penalty: with c the
+// number of times the id has been generated for the row (prompt excluded; an int16 table that saturates at 32767),
+// l = (l - f c) - p when c > 0.  With a count table, the publishing thread increments the drawn id's count
+// (saturating); every CTA of the cluster has read its counts before the draw.  Greedy rows are biased and penalised
+// too.  Both steps round to nearest explicitly (no FMA contraction), so an fp32 reference reproduces them bit for bit.
 // After temperature the filters run in transformers' processor order, with e = exp(l - max):
 //   * top-k (k per row; k <= 0 or k >= V = off): K = the tokens whose e is at least the k-th
 //     largest e, ties at the k-th value kept.  K is decided on the same 22-bit key (top 22 bits
@@ -38,10 +32,9 @@
 // and always holds the maximal tokens.  Greedy rows ignore top-k and min-p.  The branches on
 // top-k and min-p are uniform per row: a row with both off runs the phases of plain top-p.
 //
-// Performance notes: every pass over the 128k logits is
-// L2-latency bound, so logits are read 8 at a time per thread (2 x 128-bit loads in flight);
-// histogram mass is accumulated in 32.32 fixed point with native 32-bit shared-memory atomics
-// (float / 64-bit shared atomics are CAS loops).
+// Performance notes: every pass over the 128k logits is L2-latency bound, so logits are read 128 bits at a time
+// (two loads in flight per thread on plain rows); histogram mass is accumulated in 32.32 fixed point with native
+// 32-bit shared-memory atomics (float / 64-bit shared atomics are CAS loops).
 #include "kernels.h"
 
 #include "common.cuh"
@@ -50,37 +43,53 @@
 namespace b2b {
 
 constexpr int SAMP_THREADS = 1024;
-constexpr int NBINS = 4096;
 
 __device__ __forceinline__ uint32_t hash_u32(uint32_t x) {
   x ^= x >> 16; x *= 0x7feb352dU; x ^= x >> 15; x *= 0x846ca68bU; x ^= x >> 16;
   return x;
 }
 
-// logit -> (soft-cap) -> repetition penalty -> temperature
-__device__ __forceinline__ float transform(float l, bool is_seen, float pen, float inv_temp, float cap) {
+// logit -> (soft-cap) -> (+ bias b) -> repetition penalty -> (presence / frequency penalty) -> temperature, with the
+// bias and count steps compiled in only for the row kinds that read them
+template <bool BIAS, bool COUNTS>
+__device__ __forceinline__ float transform(float l, float b, bool is_seen, int c, float pen, float pres, float freq,
+                                           float inv_temp, float cap) {
   if (cap > 0.f) l = cap * tanhf(l / cap);
+  if constexpr (BIAS) l = __fadd_rn(l, b);
   if (is_seen) l = l > 0.f ? l / pen : l * pen;
+  if constexpr (COUNTS) {
+    if (c > 0) l = __fsub_rn(__fsub_rn(l, __fmul_rn(freq, static_cast<float>(c))), pres);
+  }
   return l * inv_temp;
 }
 
-// transform() with the presence / frequency penalty between the repetition penalty and temperature
-__device__ __forceinline__ float transform_pf(float l, bool is_seen, int c, float pen, float pres, float freq,
-                                             float inv_temp, float cap) {
-  if (cap > 0.f) l = cap * tanhf(l / cap);
-  if (is_seen) l = l > 0.f ? l / pen : l * pen;
-  if (c > 0) l = __fsub_rn(__fsub_rn(l, __fmul_rn(freq, static_cast<float>(c))), pres);
-  return l * inv_temp;
-}
+// phase-1 row kinds, chosen per row (see phase 1 in sample_kernel)
+enum RowKind { ROW_PLAIN, ROW_COUNTED, ROW_BIASED };
+template <RowKind K>
+struct Row { static constexpr RowKind value = K; };
 
-// transform_pf() with the logit bias b added right after soft-cap (b = 0 for an unlisted id)
-__device__ __forceinline__ float transform_bias(float l, float b, bool is_seen, int c, float pen, float pres,
-                                                float freq, float inv_temp, float cap) {
-  if (cap > 0.f) l = cap * tanhf(l / cap);
-  l = __fadd_rn(l, b);
-  if (is_seen) l = l > 0.f ? l / pen : l * pen;
-  if (c > 0) l = __fsub_rn(__fsub_rn(l, __fmul_rn(freq, static_cast<float>(c))), pres);
-  return l * inv_temp;
+// butterfly max / argmax over the warp; on equal values the lower id wins.  The test has no short-circuit, so that it
+// compiles to selects rather than branches.
+__device__ __forceinline__ void warp_argmax(float& mx, int& amx) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, amx, o);
+    if ((om > mx) | ((om == mx) & (oi < amx))) { mx = om; amx = oi; }
+  }
+}
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+// inclusive prefix sum over the lanes of the warp
+template <typename T>
+__device__ __forceinline__ T warp_scan(T v, int lane) {
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+  return v;
 }
 
 constexpr int SBINS = 2048;          // histogram bins per level (11 + 11 bits of the 28-bit key)
@@ -204,126 +213,84 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
 
   const int nbias = p.bias_n ? min(p.bias_n[bb], p.bias_stride) : 0;
 
-  // ---- phase 1: L2 -> (soft-cap, bias, penalties, temperature) -> shared memory; running max / argmax
+  // ---- phase 1: L2 -> transform() -> shared memory, with a running max / argmax.  Each thread visits its ids in
+  // increasing order and keeps the first maximum, so ties go to the lowest id.  The row kind is uniform per row and
+  // decides which steps of transform() are compiled in and what the pass reads beside the logits and `seen`:
+  //   * biased (nbias > 0): the bias staged in the ebuf slot that the transformed logit then overwrites, and the
+  //     counts when cnt != nullptr; one quad (4 ids) per thread per iteration;
+  //   * counted (cnt != nullptr): the 4 counts of a quad in one aligned 8-byte load; one quad per iteration;
+  //   * plain: two quads per iteration, so two 128-bit loads are in flight.
   float mx = -INFINITY; int amx = 0;
+  auto phase1 = [&](auto kind) {
+    constexpr RowKind K = decltype(kind)::value;
+    constexpr bool BIAS = K == ROW_BIASED;
+    constexpr int Q = K == ROW_PLAIN ? 2 : 1;                 // quads per thread per iteration
+    const bool has_cnt = K == ROW_COUNTED || (BIAS && cnt != nullptr);
+    auto take = [&](int i, float raw, float bias, uint32_t sw, int c) {
+      const float l = transform<BIAS, K != ROW_PLAIN>(raw, bias, (sw >> (i & 31)) & 1u, c, pen, pres, freq, inv_temp,
+                                                      cap);
+      ebuf[i - lo] = l;
+      if (l > mx) { mx = l; amx = i; }
+    };
+    for (int q = tid; q < n4; q += Q * SAMP_THREADS) {
+      float a[Q][4] = {};
+      // vec_ok outermost: the 128-bit loads of all Q quads issue back to back
+      if (vec_ok) {
+#pragma unroll
+        for (int u = 0; u < Q; ++u) {
+          if (u > 0 && q + u * SAMP_THREADS >= n4) break;
+          const int i0 = lo + 4 * (q + u * SAMP_THREADS);
+          const float4 va = *reinterpret_cast<const float4*>(logits + i0);
+          a[u][0] = va.x; a[u][1] = va.y; a[u][2] = va.z; a[u][3] = va.w;
+        }
+      } else {
+#pragma unroll
+        for (int u = 0; u < Q; ++u) {
+          if (u > 0 && q + u * SAMP_THREADS >= n4) break;
+          const int i0 = lo + 4 * (q + u * SAMP_THREADS);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) a[u][k] = logits[i0 + k];
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < Q; ++u) {
+        const int qu = q + u * SAMP_THREADS, i0 = lo + 4 * qu;
+        if (u > 0 && qu >= n4) break;
+        const float4 bv = BIAS ? reinterpret_cast<const float4*>(ebuf)[qu] : make_float4(0.f, 0.f, 0.f, 0.f);
+        const uint2 cw = has_cnt ? *reinterpret_cast<const uint2*>(cnt + i0) : make_uint2(0u, 0u);
+        const uint32_t sw = seen_r ? seen_r[i0 >> 5] : 0u;
+        take(i0, a[u][0], bv.x, sw, static_cast<int16_t>(cw.x & 0xFFFFu));
+        take(i0 + 1, a[u][1], bv.y, sw, static_cast<int16_t>(cw.x >> 16));
+        take(i0 + 2, a[u][2], bv.z, sw, static_cast<int16_t>(cw.y & 0xFFFFu));
+        take(i0 + 3, a[u][3], bv.w, sw, static_cast<int16_t>(cw.y >> 16));
+      }
+    }
+    for (int i = lo + 4 * n4 + tid; i < hi; i += SAMP_THREADS)
+      take(i, logits[i], BIAS ? ebuf[i - lo] : 0.f, seen_r ? seen_r[i >> 5] : 0u, has_cnt ? cnt[i] : 0);
+  };
   if (nbias > 0) {
-    // biased row: stage the bias of the ids this CTA owns in its slice (0 for the others)
+    // stage the bias of the ids this CTA owns in its slice (0 for the others)
     for (int j = tid; j < n; j += SAMP_THREADS) ebuf[j] = 0.f;
     __syncthreads();
-    const int* bid = p.bias_ids + static_cast<size_t>(bb) * p.bias_stride;
-    const float* bval = p.bias_vals + static_cast<size_t>(bb) * p.bias_stride;
+    const size_t row = static_cast<size_t>(bb) * p.bias_stride;
     for (int j = tid; j < nbias; j += SAMP_THREADS) {
-      const int id = bid[j];
-      if (id >= lo && id < hi) ebuf[id - lo] = bval[j];
+      const int id = p.bias_ids[row + j];
+      if (id >= lo && id < hi) ebuf[id - lo] = p.bias_vals[row + j];
     }
     __syncthreads();
-    // 4 ids per iteration: their staged biases in one 16-byte shared load, their counts (penalised rows) in one
-    // aligned 8-byte load
-    auto take = [&](int i, float raw, float bias, uint32_t sw, int c) {
-      const float l = transform_bias(raw, bias, (sw >> (i & 31)) & 1u, c, pen, pres, freq, inv_temp, cap);
-      ebuf[i - lo] = l;
-      if (l > mx) { mx = l; amx = i; }
-    };
-    for (int q = tid; q < n4; q += SAMP_THREADS) {
-      const int i0 = lo + 4 * q;
-      float a[4];
-      if (vec_ok) {
-        const float4 va = *reinterpret_cast<const float4*>(logits + i0);
-        a[0] = va.x; a[1] = va.y; a[2] = va.z; a[3] = va.w;
-      } else {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) a[k] = logits[i0 + k];
-      }
-      const float4 bv = reinterpret_cast<const float4*>(ebuf)[q];
-      const uint2 cw = cnt ? *reinterpret_cast<const uint2*>(cnt + i0) : make_uint2(0u, 0u);
-      const uint32_t sa = seen_r ? seen_r[i0 >> 5] : 0u;
-      take(i0, a[0], bv.x, sa, static_cast<int16_t>(cw.x & 0xFFFFu));
-      take(i0 + 1, a[1], bv.y, sa, static_cast<int16_t>(cw.x >> 16));
-      take(i0 + 2, a[2], bv.z, sa, static_cast<int16_t>(cw.y & 0xFFFFu));
-      take(i0 + 3, a[3], bv.w, sa, static_cast<int16_t>(cw.y >> 16));
-    }
-    for (int i = lo + 4 * n4 + tid; i < hi; i += SAMP_THREADS)
-      take(i, logits[i], ebuf[i - lo], seen_r ? seen_r[i >> 5] : 0u, cnt ? cnt[i] : 0);
+    phase1(Row<ROW_BIASED>{});
   } else if (cnt != nullptr) {
-    // penalised row: 4 ids per iteration, their counts in one aligned 8-byte load
-    auto take = [&](int i, float raw, uint32_t sw, int c) {
-      const float l = transform_pf(raw, (sw >> (i & 31)) & 1u, c, pen, pres, freq, inv_temp, cap);
-      ebuf[i - lo] = l;
-      if (l > mx) { mx = l; amx = i; }
-    };
-    for (int q = tid; q < n4; q += SAMP_THREADS) {
-      const int i0 = lo + 4 * q;
-      float a[4];
-      if (vec_ok) {
-        const float4 va = *reinterpret_cast<const float4*>(logits + i0);
-        a[0] = va.x; a[1] = va.y; a[2] = va.z; a[3] = va.w;
-      } else {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) a[k] = logits[i0 + k];
-      }
-      const uint2 cw = *reinterpret_cast<const uint2*>(cnt + i0);
-      const uint32_t sa = seen_r ? seen_r[i0 >> 5] : 0u;
-      take(i0, a[0], sa, static_cast<int16_t>(cw.x & 0xFFFFu));
-      take(i0 + 1, a[1], sa, static_cast<int16_t>(cw.x >> 16));
-      take(i0 + 2, a[2], sa, static_cast<int16_t>(cw.y & 0xFFFFu));
-      take(i0 + 3, a[3], sa, static_cast<int16_t>(cw.y >> 16));
-    }
-    for (int i = lo + 4 * n4 + tid; i < hi; i += SAMP_THREADS)
-      take(i, logits[i], seen_r ? seen_r[i >> 5] : 0u, cnt[i]);
+    phase1(Row<ROW_COUNTED>{});
   } else {
-    auto take = [&](int i, float raw, uint32_t sw) {
-      const float l = transform(raw, (sw >> (i & 31)) & 1u, pen, inv_temp, cap);
-      ebuf[i - lo] = l;
-      if (l > mx) { mx = l; amx = i; }
-    };
-    for (int q = tid; q < n4; q += 2 * SAMP_THREADS) {
-      const int q2 = q + SAMP_THREADS;
-      const bool has2 = q2 < n4;
-      const int i0 = lo + 4 * q, i1 = lo + 4 * q2;
-      float a[4], c[4] = {0.f, 0.f, 0.f, 0.f};
-      if (vec_ok) {
-        const float4 va = *reinterpret_cast<const float4*>(logits + i0);
-        a[0] = va.x; a[1] = va.y; a[2] = va.z; a[3] = va.w;
-        if (has2) {
-          const float4 vc = *reinterpret_cast<const float4*>(logits + i1);
-          c[0] = vc.x; c[1] = vc.y; c[2] = vc.z; c[3] = vc.w;
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) a[k] = logits[i0 + k];
-        if (has2) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) c[k] = logits[i1 + k];
-        }
-      }
-      const uint32_t sa = seen_r ? seen_r[i0 >> 5] : 0u;
-      const uint32_t sc = (seen_r && has2) ? seen_r[i1 >> 5] : 0u;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) take(i0 + k, a[k], sa);
-      if (has2) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) take(i1 + k, c[k], sc);
-      }
-    }
-    for (int i = lo + 4 * n4 + tid; i < hi; i += SAMP_THREADS) take(i, logits[i], seen_r ? seen_r[i >> 5] : 0u);
+    phase1(Row<ROW_PLAIN>{});
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float om = __shfl_xor_sync(0xffffffffu, mx, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, amx, o);
-    if (om > mx || (om == mx && oi < amx)) { mx = om; amx = oi; }
-  }
+  warp_argmax(mx, amx);
   if (lane == 0) { S.red_f[warp] = mx; S.red_i[warp] = amx; }
   __syncthreads();
   cluster_wait_acquire();            // all CTAs of the cluster are running (pairs with the arrive at kernel entry)
   if (warp == 0) {
     mx = S.red_f[lane]; amx = S.red_i[lane];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float om = __shfl_xor_sync(0xffffffffu, mx, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, amx, o);
-      if (om > mx || (om == mx && oi < amx)) { mx = om; amx = oi; }
-    }
+    warp_argmax(mx, amx);
     if (lane < CS) {       // every peer (and this CTA) gets this CTA's partial
       st_dsmem_f32(mapa_smem(smem_u32(&S.cmax[r]), lane), mx);
       st_dsmem_u32(mapa_smem(smem_u32(&S.camx[r]), lane), static_cast<uint32_t>(amx));
@@ -339,6 +306,22 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
     if (r == 0 && tid == 0) publish(token);
     return;
   }
+
+  // sum of v over the cluster: each CTA's total goes to slot[r] of every CTA, and after the cluster barrier each CTA
+  // adds the CS slots in rank order, so all of them get the same sum
+  auto cluster_total = [&](unsigned long long v, unsigned long long* slot) {
+    v = warp_sum(v);
+    if (lane == 0) S.red_u[warp] = v;
+    __syncthreads();
+    if (warp == 0) {
+      const unsigned long long z = warp_sum(S.red_u[lane]);
+      if (lane < CS) st_dsmem_u64(mapa_smem(smem_u32(&slot[r]), lane), z);
+    }
+    cluster_sync_all();
+    unsigned long long t = 0ull;
+    for (int c = 0; c < CS; ++c) t += slot[c];
+    return t;
+  };
 
   // ---- phase 2: e = exp(l - max) in place; level-1 histogram (top 11 key bits) and partition function
   unsigned long long zsum = 0ull;
@@ -364,17 +347,7 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
       hist_add(S.h1_lo, S.h1_hi, dkey(e) >> 17, f);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) zsum += __shfl_xor_sync(0xffffffffu, zsum, o);
-  if (lane == 0) S.red_u[warp] = zsum;
-  __syncthreads();
-  if (warp == 0) {
-    unsigned long long z = S.red_u[lane];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
-    if (lane < CS) st_dsmem_u64(mapa_smem(smem_u32(&S.cz[r]), lane), z);
-  }
-  cluster_sync_all();
+  unsigned long long Z = cluster_total(zsum, S.cz);
 
   // cluster-wide histogram -> S.merged (every CTA computes the same sum), then a top-down search for the
   // highest bin whose suffix mass (plus `carry`) reaches `need`.  Results: s_i[0] = bin, s_u[0] = mass above it.
@@ -406,9 +379,7 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
     if (warp == 0) {
       // lane l looks at warp-chunk 31 - l (highest bins first)
       const unsigned long long v = S.wsum[31 - lane];
-      unsigned long long pre = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, pre, o); if (lane >= o) pre += t; }
+      const unsigned long long pre = warp_scan(v, lane);
       const unsigned ball = __ballot_sync(0xffffffffu, carry + pre >= need);
       int found = -1;
       unsigned long long above = carry;
@@ -418,9 +389,7 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
         const int cbase = (31 - l0) * 64;
         for (int base = cbase + 32; base >= cbase && found < 0; base -= 32) {
           const unsigned long long bv = S.merged[base + (31 - lane)];
-          unsigned long long bp = bv;
-#pragma unroll
-          for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, bp, o); if (lane >= o) bp += t; }
+          const unsigned long long bp = warp_scan(bv, lane);
           const unsigned hit = __ballot_sync(0xffffffffu, run + bp >= need);
           if (hit) {
             const int l1 = __ffs(hit) - 1;
@@ -435,9 +404,6 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
     }
     __syncthreads();
   };
-
-  unsigned long long Z = 0ull;
-  for (int c = 0; c < CS; ++c) Z += S.cz[c];
 
   // ---- top-k (row-uniform): the 22-bit key prefix thr_k of the k-th largest e from two count levels, then
   // Z = Z_K, the mass of {key >= thr_k}.  The level-2 arrays are idle until phase 3 and hold the counts.
@@ -463,19 +429,7 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
       const float e = ebuf[j];
       if (dkey(e) >= thr_k) zk += fx32(e);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) zk += __shfl_xor_sync(0xffffffffu, zk, o);
-    if (lane == 0) S.red_u[warp] = zk;
-    __syncthreads();
-    if (warp == 0) {
-      unsigned long long z = S.red_u[lane];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
-      if (lane < CS) st_dsmem_u64(mapa_smem(smem_u32(&S.czk[r]), lane), z);
-    }
-    cluster_sync_all();               // also: no peer reads this CTA's count histograms any more
-    Z = 0ull;
-    for (int c = 0; c < CS; ++c) Z += S.czk[c];
+    Z = cluster_total(zk, S.czk);     // its cluster barrier also ends every peer's reads of the count histograms
     for (int i = tid; i < SBINS; i += SAMP_THREADS) { S.h2_lo[i] = 0u; S.h2_hi[i] = 0u; }
     // the __syncthreads inside the level-1 search below orders these stores before phase 3
   }
@@ -529,15 +483,12 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
     for (int j = c0 + 4 * nq + lane; j < c1; j += 32)
       if (dkey(ebuf[j]) >= thr) mine += ebuf[j];
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
+  mine = warp_sum(mine);
   if (lane == 0) S.wtot[warp] = mine;
   __syncthreads();
   // inclusive prefix over the 32 warp totals (every warp computes the same values)
   const float wt = S.wtot[lane];
-  float wpre = wt;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const float t = __shfl_up_sync(0xffffffffu, wpre, o); if (lane >= o) wpre += t; }
+  const float wpre = warp_scan(wt, lane);
   const float cta_total = __shfl_sync(0xffffffffu, wpre, 31);
   if (warp == 0 && lane < CS) st_dsmem_f32(mapa_smem(smem_u32(&S.ctot[r]), lane), cta_total);
   cluster_sync_all();                 // last remote access of the kernel (also fences the DSMEM histogram reads)
@@ -574,9 +525,7 @@ __global__ void __launch_bounds__(SAMP_THREADS, 1) sample_kernel(const SamplePar
     const int j = base + lane;
     float v = 0.f;
     if (j < c1) { const float e = ebuf[j]; if (dkey(e) >= thr) v = e; }
-    float pre = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const float t = __shfl_up_sync(0xffffffffu, pre, o); if (lane >= o) pre += t; }
+    const float pre = warp_scan(v, lane);
     const unsigned kept = __ballot_sync(0xffffffffu, v > 0.f);
     if (kept) last_kept = base + (31 - __clz(kept));
     const unsigned hit = __ballot_sync(0xffffffffu, v > 0.f && run + pre > target);
